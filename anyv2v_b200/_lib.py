@@ -1,13 +1,13 @@
 """ctypes loader for the C-ABI library (include/anyv2v_b200.h).
 
 There is deliberately no fallback: if ``libanyv2v_b200.so`` is missing or a call fails, the product path raises.
-Build it with ``python -c "import __graft_entry__ as g; g.build()"`` (nvcc, sm_100a).
+Build it with ``python -c "import __graft_entry__ as g; g.build()"`` (nvcc, sm_90a).
 """
 from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import c_longlong, POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int64, c_void_p
+from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("AV2V_LIB") or os.path.join(_HERE, "lib", "libanyv2v_b200.so")  # AV2V_LIB: bring-up builds
@@ -69,8 +69,6 @@ EXPORTS = {
     "av2v_layernorm_f16": (c_int, [POINTER(LayerNormArgs), c_void_p]),
     "av2v_attn_pnp_f16": (c_int, [POINTER(AttnArgs), c_void_p]),
     "av2v_tattn_fused_f16": (c_int, [POINTER(TAttnFusedArgs), c_void_p]),
-    "av2v_gemm_debug_timers": (c_int, [c_void_p]),  # diagnostics
-    "av2v_tmap_cache_stats": (c_int, [POINTER(c_longlong), POINTER(c_longlong), POINTER(c_int)]),  # diagnostics
 }
 
 _lib = None

@@ -1,44 +1,7 @@
-// C-ABI plumbing: version, thread-local error text, device query, the tensor-map descriptor cache.
-#include <mutex>
-#include <unordered_map>
-
+// C-ABI plumbing: version, thread-local error text, device query.
 #include "host_util.cuh"
 
 namespace av2v {
-
-// ------------------------------------------------------------------ CUtensorMap cache (see make_tmap_f16, host_util.cuh)
-namespace {
-struct TmapKeyHash {
-  size_t operator()(const TmapKey& k) const {  // FNV-1a over the raw bytes (the key is memset before it is filled)
-    const unsigned char* p = reinterpret_cast<const unsigned char*>(&k);
-    uint64_t h = 1469598103934665603ull;
-    for (size_t i = 0; i < sizeof(TmapKey); ++i) h = (h ^ p[i]) * 1099511628211ull;
-    return static_cast<size_t>(h);
-  }
-};
-constexpr size_t kTmapCacheMax = 16384;  // ~3 MB; a UNet step touches a few hundred distinct descriptors
-std::mutex g_tmap_mu;
-std::unordered_map<TmapKey, CUtensorMap, TmapKeyHash> g_tmap_cache;
-long long g_tmap_hits = 0, g_tmap_misses = 0;
-}  // namespace
-
-bool tmap_cache_lookup(const TmapKey& key, CUtensorMap* out) {
-  std::lock_guard<std::mutex> lock(g_tmap_mu);
-  auto it = g_tmap_cache.find(key);
-  if (it == g_tmap_cache.end()) {
-    ++g_tmap_misses;
-    return false;
-  }
-  ++g_tmap_hits;
-  *out = it->second;
-  return true;
-}
-
-void tmap_cache_insert(const TmapKey& key, const CUtensorMap& m) {
-  std::lock_guard<std::mutex> lock(g_tmap_mu);
-  if (g_tmap_cache.size() >= kTmapCacheMax) g_tmap_cache.clear();  // bounded: start over rather than grow
-  g_tmap_cache.emplace(key, m);
-}
 
 char* last_error_buf() {
   static thread_local char buf[512] = {0};
@@ -48,10 +11,10 @@ char* last_error_buf() {
 int sm_count_cached() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -63,14 +26,6 @@ extern "C" int av2v_abi_version(void) { return 1; }
 
 extern "C" const char* av2v_last_error(void) { return av2v::last_error_buf(); }
 
-extern "C" int av2v_tmap_cache_stats(long long* hits, long long* misses, int* entries) {
-  std::lock_guard<std::mutex> lock(av2v::g_tmap_mu);
-  if (hits) *hits = av2v::g_tmap_hits;
-  if (misses) *misses = av2v::g_tmap_misses;
-  if (entries) *entries = static_cast<int>(av2v::g_tmap_cache.size());
-  return AV2V_OK;
-}
-
 extern "C" int av2v_device_info(int* sm_count, int* cc_major, int* cc_minor) {
   int dev = 0;
   AV2V_CHECK_CUDA(cudaGetDevice(&dev));
@@ -81,6 +36,6 @@ extern "C" int av2v_device_info(int* sm_count, int* cc_major, int* cc_minor) {
   if (sm_count) *sm_count = sm;
   if (cc_major) *cc_major = maj;
   if (cc_minor) *cc_minor = min;
-  if (maj != 10) return av2v::fail(AV2V_ENOSUP, "device compute capability %d.%d is not sm_100", maj, min);
+  if (maj != 9 || min != 0) return av2v::fail(AV2V_ENOSUP, "device compute capability %d.%d is not sm_90", maj, min);
   return AV2V_OK;
 }

@@ -1,0 +1,507 @@
+// PnP attention core on wgmma (sm_90a), head_dim 64: av2v_attn_pnp_f16 (spatial / cross / temporal attention, with the PnP
+// Q/K injection folded in) and av2v_tattn_fused_f16 (temporal self-attention with the Q/K/V projection in the same kernel).
+//
+// A CTA holds 128 query slots, two warpgroups of 64.  Per 64-key tile a warpgroup computes S = Q K^T with wgmma.m64n64k16
+// (Q and K as 128-byte-swizzled K-major tiles in shared memory), runs the online softmax on its accumulator registers
+// (running max / sum per row, base-2 exponentials; a quarter of them on the FMA pipe, ex2_poly), converts P to fp16 in
+// registers — the accumulator layout of S is the A-fragment layout of the next wgmma — and accumulates O += P V with V read
+// MN-major ([keys][64], 64 contiguous) from shared memory.  With n_v = 3 (injected step) ONE P feeds the V of all three
+// branches.  K / V tiles are double-buffered with cp.async.
+//
+// Query slots map to token rows by mode:
+//   rows   : slot i of q tile qt -> token qt * 128 + i of sequence b; keys = the b / kv_batch_div-th key sequence.
+//   frames : tokens are frame-major [clips][F][HW][*].  F <= 128 (F | 128): a CTA packs 128 / F pixels of a clip, slot i ->
+//            (pixel i / F, frame i % F), and the keys are the same 128 slots masked to the slot's own pixel.  F % 128 == 0:
+//            one pixel, slot i -> frame ft * 128 + i, keys = all F frames of the pixel.
+#include "host_util.cuh"
+#include "ptx.cuh"
+
+namespace av2v {
+namespace {
+
+constexpr int HD = 64;
+constexpr int kThreads = 256;
+constexpr int kTile = 64 * 128;  // bytes of a 64-row, 64-column fp16 tile
+
+// 16-byte chunk loads of `rows` tile rows (64 fp16 each) into a swizzled tile, all 256 threads; row_ptr(r) -> source or null
+// (a null row is zero-filled; `any` is a valid address handed to cp.async, which then reads nothing)
+template <typename RowPtr>
+__device__ __forceinline__ void load_tile(uint32_t dst, int rows, const __half* any, RowPtr row_ptr) {
+  for (int c = threadIdx.x; c < rows * 8; c += kThreads) {
+    const int r = c >> 3, ch = c & 7;
+    const __half* src = row_ptr(r);
+    cp_async16(dst + sw128_offset(r, ch), src ? src + ch * 8 : any, src != nullptr);
+  }
+}
+
+// Online-softmax attention of one warpgroup's 64 query rows against one 64-key tile.  keep(row, key) masks scores;
+// m / l: running max (base-2 scaled) and partial sum of the thread's rows r, r + 8.
+template <int NV, typename Keep>
+__device__ __forceinline__ void attn_tile(uint32_t q_wg, uint32_t k_tile, const uint32_t (&v_tile)[NV], float (&o)[NV][32],
+                                          float (&m)[2], float (&l)[2], float scale_log2, Keep keep) {
+  float s[32];
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < HD / 16; ++k) wgmma_m64n64_ss<0>(s, sw128_desc(q_wg + k * 32), sw128_desc(k_tile + k * 32), k > 0);
+  wgmma_commit();
+  wgmma_wait<0>();
+  reg_fence(s);
+
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    const float v = keep(acc_row(i), acc_col(i)) ? s[i] * scale_log2 : -INFINITY;
+    s[i] = v;
+    mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], v);
+  }
+  float corr[2], ref[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+    mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+    const float mn = fmaxf(m[h], mx[h]);
+    ref[h] = mn == -INFINITY ? 0.f : mn;  // a row with every key masked so far keeps p = 0
+    corr[h] = ex2_approx(m[h] - ref[h]);
+    m[h] = mn;
+    l[h] *= corr[h];
+  }
+#pragma unroll
+  for (int b = 0; b < NV; ++b)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[b][i] *= corr[(i >> 1) & 1];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    const float x = s[i] - ref[(i >> 1) & 1];
+    s[i] = ((i >> 2) & 3) == 3 ? ex2_poly(x) : ex2_approx(x);
+    l[(i >> 1) & 1] += s[i];
+  }
+  uint32_t pa[4][4];
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+    for (int r = 0; r < 4; ++r) pa[kk][r] = pack_half2(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
+  wgmma_fence();
+#pragma unroll
+  for (int b = 0; b < NV; ++b)
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_m64n64_rs<1>(o[b], pa[kk], sw128_desc(v_tile[b] + kk * 2048), 1);
+  wgmma_commit();
+  wgmma_wait<0>();
+#pragma unroll
+  for (int b = 0; b < NV; ++b) reg_fence(o[b]);
+}
+
+// O / l -> fp16, rows mapped by out_row(slot) (negative: not stored)
+template <int NV, typename OutRow>
+__device__ __forceinline__ void store_o(float (&o)[NV][32], float (&l)[2], __half* const (&obase)[NV], int wg, OutRow out_row) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
+    l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
+    l[h] = l[h] > 0.f ? 1.f / l[h] : 0.f;
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const long long orow = out_row(wg * 64 + acc_row(2 * h));
+    if (orow < 0) continue;
+#pragma unroll
+    for (int b = 0; b < NV; ++b)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int i = 4 * j + 2 * h;
+        *reinterpret_cast<uint32_t*>(obase[b] + orow + acc_col(i)) = pack_half2(o[b][i] * l[h], o[b][i + 1] * l[h]);
+      }
+  }
+}
+
+// --------------------------------------------------------------------------------------------------- av2v_attn_pnp_f16
+struct AttnP {
+  int seq_mode;
+  const __half *q, *k, *v;
+  __half* o;
+  int ldq, ldk, ldv, ldo;
+  int heads;
+  long long v_branch_stride, o_branch_stride;
+  float scale_log2;
+  int seq, seq_kv, kv_div, q_tiles;  // rows
+  int F, HW, ppt, pix_tiles, f_tiles;  // frames
+};
+
+template <int NV>
+__global__ void __launch_bounds__(kThreads) attn_kernel(const __grid_constant__ AttnP p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const uint32_t sQ = smem_u32(smem);
+  auto sK = [&](int buf) { return sQ + 2 * kTile + buf * (1 + NV) * kTile; };
+  auto sV = [&](int buf, int b) { return sK(buf) + (1 + b) * kTile; };
+  const int wg = threadIdx.x >> 7;
+
+  // item -> (sequence / pixel group, head, query tile); qrow(slot) / krow(key) give token rows, -1 for none
+  int item = blockIdx.x;
+  const bool packed = p.seq_mode == AV2V_SEQ_FRAMES && p.F <= 128;
+  int h, qt, b = 0, clip = 0, pix0 = 0, n_kv;
+  if (p.seq_mode == AV2V_SEQ_ROWS) {
+    qt = item % p.q_tiles;
+    item /= p.q_tiles;
+    h = item % p.heads;
+    b = item / p.heads;
+    n_kv = (p.seq_kv + 63) / 64;
+  } else if (packed) {
+    qt = item % p.pix_tiles;
+    item /= p.pix_tiles;
+    h = item % p.heads;
+    clip = item / p.heads;
+    pix0 = qt * p.ppt;
+    n_kv = 2;
+  } else {
+    qt = item % p.f_tiles;
+    item /= p.f_tiles;
+    h = item % p.heads;
+    item /= p.heads;
+    pix0 = item % p.HW;
+    clip = item / p.HW;
+    n_kv = p.F / 64;
+  }
+  const long long clip_row = static_cast<long long>(clip) * p.F * p.HW;
+  auto qrow = [&](int i) -> long long {
+    if (p.seq_mode == AV2V_SEQ_ROWS) {
+      const int t = qt * 128 + i;
+      return t < p.seq ? static_cast<long long>(b) * p.seq + t : -1;
+    }
+    if (packed) {
+      const int pix = pix0 + i / p.F;
+      return pix < p.HW ? clip_row + static_cast<long long>(i % p.F) * p.HW + pix : -1;
+    }
+    return clip_row + static_cast<long long>(qt * 128 + i) * p.HW + pix0;
+  };
+  auto krow = [&](int u) -> long long {  // key u of the key sequence(s)
+    if (p.seq_mode == AV2V_SEQ_ROWS)
+      return u < p.seq_kv ? static_cast<long long>(b / p.kv_div) * p.seq_kv + u : -1;
+    if (packed) {
+      const int pix = pix0 + u / p.F;
+      return pix < p.HW ? clip_row + static_cast<long long>(u % p.F) * p.HW + pix : -1;
+    }
+    return clip_row + static_cast<long long>(u) * p.HW + pix0;
+  };
+  const int hc = h * HD;
+  auto load_kv = [&](int kt, int buf) {
+    load_tile(sK(buf), 64, p.k, [&](int r) -> const __half* {
+      const long long row = krow(kt * 64 + r);
+      return row < 0 ? nullptr : p.k + row * p.ldk + hc;
+    });
+#pragma unroll
+    for (int vb = 0; vb < NV; ++vb)
+      load_tile(sV(buf, vb), 64, p.v, [&](int r) -> const __half* {
+        const long long row = krow(kt * 64 + r);
+        return row < 0 ? nullptr : p.v + vb * p.v_branch_stride + row * p.ldv + hc;
+      });
+  };
+  load_tile(sQ, 128, p.q, [&](int r) -> const __half* {
+    const long long row = qrow(r);
+    return row < 0 ? nullptr : p.q + row * p.ldq + hc;
+  });
+  load_kv(0, 0);
+  cp_async_commit();
+
+  float o[NV][32];
+#pragma unroll
+  for (int vb = 0; vb < NV; ++vb)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[vb][i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  const int nk = p.seq_mode == AV2V_SEQ_ROWS ? p.seq_kv : 1 << 30;
+  for (int kt = 0; kt < n_kv; ++kt) {
+    if (kt + 1 < n_kv) {
+      load_kv(kt + 1, (kt + 1) & 1);
+      cp_async_commit();
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+    uint32_t vt[NV];
+#pragma unroll
+    for (int vb = 0; vb < NV; ++vb) vt[vb] = sV(kt & 1, vb);
+    const int q0 = wg * 64, k0 = kt * 64;
+    if (packed) {
+      const int F = p.F;
+      attn_tile<NV>(sQ + wg * kTile, sK(kt & 1), vt, o, m, l, p.scale_log2,
+                    [&](int r, int c) { return (q0 + r) / F == (k0 + c) / F; });
+    } else {
+      attn_tile<NV>(sQ + wg * kTile, sK(kt & 1), vt, o, m, l, p.scale_log2, [&](int, int c) { return k0 + c < nk; });
+    }
+    __syncthreads();  // every warpgroup is done with this buffer before the next prefetch overwrites it
+  }
+  __half* ob[NV];
+#pragma unroll
+  for (int vb = 0; vb < NV; ++vb) ob[vb] = p.o + vb * p.o_branch_stride + hc;
+  store_o<NV>(o, l, ob, wg, [&](int i) -> long long {
+    const long long row = qrow(i);
+    return row < 0 ? -1 : row * p.ldo;
+  });
+}
+
+template <int NV>
+constexpr int attn_smem() { return 2 * kTile + 2 * (1 + NV) * kTile + 1024; }
+
+// --------------------------------------------------------------------------------------------------- av2v_tattn_fused_f16
+struct TAttnP {
+  const __half* x;
+  const __half* wqkv;
+  __half* o;
+  int ldx, ldo, F, HW, heads, Cx, ppt, pix_tiles, src_clips;
+  float scale_log2;
+};
+
+// smem: Q, K (128 x 64 each), V per branch (128 x 64), then the projection ring: 2 stages x (A 128 x 64 + up to 3 W 64 x 64)
+template <int NV>
+constexpr int tattn_smem() { return (2 + NV) * 2 * kTile + 2 * (2 * kTile + 3 * kTile) + 1024; }
+
+// acc[part] (64 x 64 per warpgroup) = x rows of the 128 slots (xrow(slot)) @ W rows w_row0[part] .. + 64, over Cx
+template <int NP, typename XRow>
+__device__ __forceinline__ void project(const TAttnP& p, XRow xrow, const int (&w_row0)[NP], uint32_t ring, float (&acc)[NP][32]) {
+  const int wg = threadIdx.x >> 7;
+  const uint32_t stage_bytes = 2 * kTile + 3 * kTile;
+  auto load = [&](int kb, int st) {
+    const uint32_t base = ring + st * stage_bytes;
+    const int k0 = kb * 64;
+    load_tile(base, 128, p.x, [&](int r) -> const __half* {
+      const long long row = xrow(r);
+      return row < 0 ? nullptr : p.x + row * p.ldx + k0;
+    });
+#pragma unroll
+    for (int q = 0; q < NP; ++q)
+      load_tile(base + (2 + q) * kTile, 64, p.wqkv,
+                [&](int r) -> const __half* { return p.wqkv + static_cast<long long>(w_row0[q] + r) * p.Cx + k0; });
+  };
+#pragma unroll
+  for (int q = 0; q < NP; ++q)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[q][i] = 0.f;
+  const int nk = p.Cx / 64;
+  load(0, 0);
+  cp_async_commit();
+  for (int kb = 0; kb < nk; ++kb) {
+    if (kb + 1 < nk) {
+      load(kb + 1, (kb + 1) & 1);
+      cp_async_commit();
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+    const uint32_t base = ring + (kb & 1) * stage_bytes;
+    wgmma_fence();
+#pragma unroll
+    for (int q = 0; q < NP; ++q)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n64_ss<0>(acc[q], sw128_desc(base + wg * kTile + k * 32), sw128_desc(base + (2 + q) * kTile + k * 32), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int q = 0; q < NP; ++q) reg_fence(acc[q]);
+    __syncthreads();
+  }
+}
+
+// accumulator (64 x 64 of warpgroup wg) -> fp16 into the swizzled 128 x 64 tile at `tile` (the projection GEMM's rounding)
+__device__ __forceinline__ void acc_to_tile(const float (&acc)[32], uint32_t tile, int wg) {
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    const int r = wg * 64 + acc_row(i), c = acc_col(i);
+    const uint32_t addr = tile + sw128_offset(r, c >> 3) + (c & 7) * 2;
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_half2(acc[i], acc[i + 1])) : "memory");
+  }
+}
+
+template <int NV>
+__global__ void __launch_bounds__(kThreads) tattn_fused_kernel(const __grid_constant__ TAttnP p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const uint32_t sQ = smem_u32(smem), sK = sQ + 2 * kTile;
+  auto sV = [&](int b) { return sQ + (2 + b) * 2 * kTile; };
+  const uint32_t ring = sQ + (2 + NV) * 2 * kTile;
+  const int wg = threadIdx.x >> 7;
+
+  int item = blockIdx.x;
+  const int pt = item % p.pix_tiles;
+  item /= p.pix_tiles;
+  const int h = item % p.heads;
+  const int clip = item / p.heads;  // source clip (n_v = 3) or clip
+  const int pix0 = pt * p.ppt, F = p.F, C = p.heads * HD;
+  auto row_in = [&](int c, int i) -> long long {
+    const int pix = pix0 + i / F;
+    return pix < p.HW ? (static_cast<long long>(c) * F + i % F) * p.HW + pix : -1;
+  };
+  {
+    float acc[3][32];
+    const int w3[3] = {h * HD, C + h * HD, 2 * C + h * HD};
+    project<3>(p, [&](int i) { return row_in(clip, i); }, w3, ring, acc);
+    acc_to_tile(acc[0], sQ, wg);
+    acc_to_tile(acc[1], sK, wg);
+    acc_to_tile(acc[2], sV(0), wg);
+  }
+#pragma unroll
+  for (int b = 1; b < NV; ++b) {
+    float acc[1][32];
+    const int w1[1] = {2 * C + h * HD};
+    project<1>(p, [&](int i) { return row_in(clip + b * p.src_clips, i); }, w1, ring, acc);
+    acc_to_tile(acc[0], sV(b), wg);
+  }
+  fence_proxy_async_smem();
+  __syncthreads();
+
+  float o[NV][32];
+#pragma unroll
+  for (int b = 0; b < NV; ++b)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[b][i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  const int q0 = wg * 64;
+  // sequences of <= 64 frames never cross the 64-slot halves: each warpgroup then needs only its own key half.  The tile index
+  // is data, not control flow, so both warpgroups issue the same wgmma sequence (no divergent path around the wgmma).
+  const int n_kt = F <= 64 ? 1 : 2;
+  for (int it = 0; it < n_kt; ++it) {
+    const int kt = F <= 64 ? wg : it;
+    const int k0 = kt * 64;
+    uint32_t vt[NV];
+#pragma unroll
+    for (int b = 0; b < NV; ++b) vt[b] = sV(b) + kt * kTile;
+    attn_tile<NV>(sQ + wg * kTile, sK + kt * kTile, vt, o, m, l, p.scale_log2,
+                  [&](int r, int c) { return (q0 + r) / F == (k0 + c) / F; });
+  }
+  // branch b writes the rows of its own clip, clip + b * src_clips
+#pragma unroll
+  for (int b = 0; b < NV; ++b) {
+    float (&ob)[1][32] = *reinterpret_cast<float(*)[1][32]>(&o[b]);
+    float lb[2] = {l[0], l[1]};
+    __half* const o1[1] = {p.o + h * HD};
+    store_o<1>(ob, lb, o1, wg, [&](int i) -> long long {
+      const long long row = row_in(clip + b * p.src_clips, i);
+      return row < 0 ? -1 : row * p.ldo;
+    });
+  }
+}
+
+}  // namespace
+}  // namespace av2v
+
+using namespace av2v;
+
+extern "C" int av2v_attn_pnp_f16(const av2v_attn_args* a, av2v_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  AV2V_REQUIRE(a != nullptr, AV2V_EINVAL, "attn: null args");
+  AV2V_REQUIRE(a->q && a->k && a->v && a->o, AV2V_EINVAL, "attn: null q/k/v/o");
+  AV2V_REQUIRE(a->batch > 0 && a->seq > 0 && a->heads > 0, AV2V_EINVAL, "attn: batch/seq/heads must be positive");
+  AV2V_REQUIRE(a->n_v == 1 || a->n_v == 3, AV2V_EINVAL, "attn: n_v must be 1 or 3 (got %d)", a->n_v);
+  AV2V_REQUIRE(a->ldq % 8 == 0 && a->ldk % 8 == 0 && a->ldv % 8 == 0 && a->ldo % 8 == 0, AV2V_EALIGN,
+               "attn: row strides must be multiples of 8 elements");
+  AV2V_REQUIRE(a->ldq >= a->heads * HD && a->ldk >= a->heads * HD && a->ldv >= a->heads * HD &&
+                   a->ldo >= a->heads * HD,
+               AV2V_EINVAL, "attn: row strides must cover heads*64 columns");
+  AV2V_REQUIRE(aligned16(a->q) && aligned16(a->k) && aligned16(a->v) && aligned16(a->o), AV2V_EALIGN,
+               "attn: q/k/v/o must be 16-byte aligned");
+  AV2V_REQUIRE(a->scale > 0.f, AV2V_EINVAL, "attn: scale must be positive");
+  AV2V_REQUIRE(a->n_v == 1 || (a->v_branch_stride % 8 == 0 && a->o_branch_stride % 8 == 0), AV2V_EALIGN,
+               "attn: branch strides must be multiples of 8 elements");
+
+  AttnP p{};
+  p.seq_mode = a->seq_mode;
+  p.q = static_cast<const __half*>(a->q);
+  p.k = static_cast<const __half*>(a->k);
+  p.v = static_cast<const __half*>(a->v);
+  p.o = static_cast<__half*>(a->o);
+  p.ldq = a->ldq;
+  p.ldk = a->ldk;
+  p.ldv = a->ldv;
+  p.ldo = a->ldo;
+  p.heads = a->heads;
+  p.v_branch_stride = a->n_v == 3 ? a->v_branch_stride : 0;
+  p.o_branch_stride = a->n_v == 3 ? a->o_branch_stride : 0;
+  p.scale_log2 = a->scale * 1.4426950408889634f;
+  p.seq = a->seq;
+  p.seq_kv = a->seq_kv > 0 ? a->seq_kv : a->seq;
+  p.kv_div = a->kv_batch_div > 0 ? a->kv_batch_div : 1;
+  long long items;
+  if (a->seq_mode == AV2V_SEQ_ROWS) {
+    AV2V_REQUIRE(a->batch % p.kv_div == 0, AV2V_EINVAL, "attn: batch must be a multiple of kv_batch_div");
+    p.q_tiles = (a->seq + 127) / 128;
+    items = static_cast<long long>(a->batch) * a->heads * p.q_tiles;
+  } else if (a->seq_mode == AV2V_SEQ_FRAMES) {
+    const int F = a->seq, HW = a->HW;
+    AV2V_REQUIRE(HW > 0 && a->batch % HW == 0, AV2V_EINVAL, "attn/frames: batch must be clips*HW");
+    AV2V_REQUIRE((a->seq_kv <= 0 || a->seq_kv == a->seq) && p.kv_div == 1, AV2V_ENOSUP,
+                 "attn/frames: self-attention only (seq_kv / kv_batch_div are rows-mode options)");
+    AV2V_REQUIRE((F <= 128 && 128 % F == 0) || (F % 128 == 0), AV2V_ENOSUP,
+                 "attn/frames: F must divide 128 or be a multiple of 128 (got %d)", F);
+    const int clips = a->batch / HW;
+    p.F = F;
+    p.HW = HW;
+    if (F <= 128) {
+      p.ppt = 128 / F;
+      p.pix_tiles = (HW + p.ppt - 1) / p.ppt;
+      items = static_cast<long long>(clips) * a->heads * p.pix_tiles;
+    } else {
+      p.f_tiles = F / 128;
+      items = static_cast<long long>(clips) * HW * a->heads * p.f_tiles;
+    }
+  } else {
+    return fail(AV2V_EINVAL, "attn: unknown seq_mode %d", a->seq_mode);
+  }
+  AV2V_REQUIRE(items < (1ll << 31), AV2V_ENOSUP, "attn: too many work items");
+  static bool attr_set = false;
+  if (!attr_set) {
+    AV2V_CHECK_CUDA(cudaFuncSetAttribute(attn_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn_smem<1>()));
+    AV2V_CHECK_CUDA(cudaFuncSetAttribute(attn_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn_smem<3>()));
+    attr_set = true;
+  }
+  if (a->n_v == 3) attn_kernel<3><<<static_cast<unsigned>(items), kThreads, attn_smem<3>(), stream>>>(p);
+  else attn_kernel<1><<<static_cast<unsigned>(items), kThreads, attn_smem<1>(), stream>>>(p);
+  AV2V_CHECK_CUDA(cudaGetLastError());
+  return AV2V_OK;
+}
+
+extern "C" int av2v_tattn_fused_f16(const av2v_tattn_fused_args* a, av2v_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  AV2V_REQUIRE(a != nullptr, AV2V_EINVAL, "tattn_fused: null args");
+  AV2V_REQUIRE(a->x && a->wqkv && a->o, AV2V_EINVAL, "tattn_fused: null x / wqkv / o");
+  AV2V_REQUIRE(a->clips > 0 && a->F > 0 && a->HW > 0 && a->heads > 0 && a->Cx > 0, AV2V_EINVAL, "tattn_fused: bad shape");
+  AV2V_REQUIRE(a->F <= 128 && 128 % a->F == 0, AV2V_ENOSUP, "tattn_fused: F must divide 128 (got %d)", a->F);
+  AV2V_REQUIRE(a->Cx % 64 == 0, AV2V_ENOSUP, "tattn_fused: the input width must be a multiple of 64 (got %d)", a->Cx);
+  AV2V_REQUIRE(a->ldx % 8 == 0 && a->ldx >= a->Cx && a->ldo % 8 == 0 && a->ldo >= a->heads * HD, AV2V_EINVAL,
+               "tattn_fused: row strides must be multiples of 8 covering the rows");
+  AV2V_REQUIRE(aligned16(a->x) && aligned16(a->wqkv) && aligned16(a->o), AV2V_EALIGN, "tattn_fused: pointers must be 16-byte aligned");
+  AV2V_REQUIRE(a->scale > 0.f, AV2V_EINVAL, "tattn_fused: scale must be positive");
+  AV2V_REQUIRE(a->n_v == 1 || a->n_v == 3, AV2V_EINVAL, "tattn_fused: n_v must be 1 or 3 (got %d)", a->n_v);
+  AV2V_REQUIRE(a->n_v == 1 || a->clips % 3 == 0, AV2V_EINVAL, "tattn_fused: n_v = 3 needs clips = 3 x clips-per-branch (got %d)", a->clips);
+
+  TAttnP p{};
+  p.x = static_cast<const __half*>(a->x);
+  p.wqkv = static_cast<const __half*>(a->wqkv);
+  p.o = static_cast<__half*>(a->o);
+  p.ldx = a->ldx;
+  p.ldo = a->ldo;
+  p.F = a->F;
+  p.HW = a->HW;
+  p.heads = a->heads;
+  p.Cx = a->Cx;
+  p.ppt = 128 / a->F;
+  p.pix_tiles = (a->HW + p.ppt - 1) / p.ppt;
+  p.src_clips = a->n_v == 3 ? a->clips / 3 : a->clips;
+  p.scale_log2 = a->scale * 1.4426950408889634f;
+  const long long items = static_cast<long long>(p.src_clips) * a->heads * p.pix_tiles;
+  AV2V_REQUIRE(items < (1ll << 31), AV2V_ENOSUP, "tattn_fused: too many work items");
+  static bool attr_set = false;
+  if (!attr_set) {
+    AV2V_CHECK_CUDA(cudaFuncSetAttribute(tattn_fused_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, tattn_smem<1>()));
+    AV2V_CHECK_CUDA(cudaFuncSetAttribute(tattn_fused_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, tattn_smem<3>()));
+    attr_set = true;
+  }
+  if (a->n_v == 3) tattn_fused_kernel<3><<<static_cast<unsigned>(items), kThreads, tattn_smem<3>(), stream>>>(p);
+  else tattn_fused_kernel<1><<<static_cast<unsigned>(items), kThreads, tattn_smem<1>(), stream>>>(p);
+  AV2V_CHECK_CUDA(cudaGetLastError());
+  return AV2V_OK;
+}

@@ -153,8 +153,7 @@ layernorm_kernel(const __half* __restrict__ x, __half* __restrict__ y, const __h
 
 
 // ---------------------------------------------------------------------------------------------------- LayerNorm, C = 40 * LPR vectors
-// The product path (measured on B200, profiles/r02_probe.txt: 49.1 us = 5.1 TB/s on the 196 608 x 320 token matrix of the finest
-// level against 70.8 us for one-warp-per-row).  Every I2VGen-XL width is a multiple of 320 = 40 vectors, so LPR = C / 40 lanes (8, 16 or 32) share a row with exactly FIVE 16-byte vectors each: 32 / LPR rows per warp
+// The product path.  Every I2VGen-XL width is a multiple of 320 = 40 vectors, so LPR = C / 40 lanes (8, 16 or 32) share a row with exactly FIVE 16-byte vectors each: 32 / LPR rows per warp
 // per iteration, all lanes busy; warps are persistent (grid-stride over rows), gamma / beta are staged in shared memory once
 // per CTA, and the next iteration's vectors are loaded before the current ones are reduced.
 template <int LPR>

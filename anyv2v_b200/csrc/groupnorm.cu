@@ -3,11 +3,11 @@
 //
 //   x, y : [n_samples][rows][C] fp16;  statistics per (sample, group) over rows x (C / groups) elements
 //
-// ONE persistent kernel, one CTA per SM, built around the 126 MB L2 (round 1 ran two kernels = three HBM passes, 6 B/element):
+// ONE persistent kernel, one CTA per SM, built around the 50 MB L2 (round 1 ran two kernels = three HBM passes, 6 B/element):
 //   * the samples are cut into L2-sized CHUNKS (<= kChunkBytes of x).  For each chunk the whole grid first streams the chunk
 //     once for the statistics (phase A: HBM -> L2 -> smem), meets at a grid-wide barrier, and then streams the SAME rows again
 //     for the normalisation (phase B): that second read hits in L2, so x crosses HBM once.  A clip-level sample of the 64 x 64
-//     level (65 536 rows x 320 channels = 42 MB) is one chunk; the per-frame norms (48 samples of 2.6 MB) go 16 frames at a time.
+//     level (65 536 rows x 320 channels = 42 MB) is one sample larger than a chunk; the per-frame norms (48 samples of 2.6 MB) go 7 frames at a time.
 //     Samples larger than L2 (128-frame clips) still work — phase B then walks the chunk back to front, so its first reads
 //     hit the part of x that phase A touched last.
 //   * rows are contiguous in the channels-last layout, so a slice of rows is ONE byte range: a producer warp moves it with
@@ -25,7 +25,7 @@ constexpr int kGnMaxSlices = 512;   // slices per sample (partial-sum slots)
 constexpr int kGnMaxGroups = 64;
 constexpr int kStages = 4;
 constexpr int kStageBytes = 30 * 1024;                 // one stage = T consumer threads x U 16-byte vectors <= this
-constexpr long long kChunkBytes = 48ll << 20;          // x + y of a chunk (2 x 48 MB) stay inside the 126 MB L2
+constexpr long long kChunkBytes = 20ll << 20;          // x + y of a chunk (2 x 20 MB) stay inside the 50 MB L2
 // Two builds: <U = 3, T <= 640> and <U = 4, T <= 480> (T = consumer threads, a multiple of the vectors per row and of 32; U =
 // vectors per thread and stage).  The SiLU pass is a chain of ~10 dependent instructions per element with two MUFU ops in it
 // (~70 cycles); at the HBM rate an SM must retire ~1.5 elements per clock and sub-partition, which takes >= 100 independent
@@ -489,7 +489,7 @@ extern "C" int av2v_groupnorm_silu_f16(const av2v_groupnorm_args* a, av2v_stream
   p.n_chunks = (a->n_samples + p.chunk_samples - 1) / p.chunk_samples;
 
   // slices per sample: the chunk's items (chunk_samples x slices) should fill whole rounds of the grid (one CTA per SM) — 48
-  // frames go 16 at a time, and 16 x 37 slices = 592 = 4 x 148 items — with at least two pipeline stages per slice when the
+  // frames go 7 at a time, and 7 x 37 slices = 259 ~ 2 x 132 items — with at least two pipeline stages per slice when the
   // sample is that long.  Score = fill of the last round, minus a little per extra round (per-item fold / barrier overhead).
   const int sms = sm_count_cached();
   int max_s = a->rows / (2 * p.stage_rows);

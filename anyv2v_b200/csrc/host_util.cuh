@@ -1,4 +1,4 @@
-// Host-side helpers shared by the C-ABI translation units: error text, argument checks, TMA descriptor encoding.
+// Host-side helpers shared by the C-ABI translation units: error text, argument checks.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -37,109 +37,6 @@ inline int fail(int code, const char* fmt, ...) {
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-// cuTensorMapEncodeTiled through the runtime's driver entry point (no link-time libcuda dependency, so the
-// library also loads on a box without a driver — needed for the CPU-side symbol-export test).
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-inline PFN_encodeTiled get_encode_tiled() {
-  static PFN_encodeTiled fn = nullptr;
-  if (fn) return fn;
-  void* p = nullptr;
-  cudaDriverEntryPointQueryResult q;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess ||
-      q != cudaDriverEntryPointSuccess)
-    return nullptr;
-  fn = reinterpret_cast<PFN_encodeTiled>(p);
-  return fn;
-}
-
-// fp16 tiled tensor map with 128-byte swizzle; dims/box innermost first; strides (bytes) for dims 1..rank-1.
-// Descriptors are CACHED (SURVEY 8b: "library allocates nothing persistent except cached CUtensorMaps keyed by (ptr, shape)"):
-// the key is everything the encoding depends on — base pointer, rank, dims, strides, box, swizzle; the table lives in abi.cu
-// behind a mutex (the only mutable global state of the library besides the thread-local error text) and is bounded.  A step of
-// the UNet issues ~1000 launches with 3-5 descriptors each over a few hundred distinct (pointer, shape) pairs: after the first
-// step every launch is a table hit instead of 3-5 driver calls.
-struct TmapKey {
-  uint64_t base;
-  uint64_t dims[5];
-  uint64_t strides[4];
-  uint32_t box[5];
-  uint32_t estr[5];  // element (traversal) strides
-  uint32_t rank, swizzle;
-  bool operator==(const TmapKey& o) const { return memcmp(this, &o, sizeof(TmapKey)) == 0; }
-};
-bool tmap_cache_lookup(const TmapKey& key, CUtensorMap* out);   // abi.cu
-void tmap_cache_insert(const TmapKey& key, const CUtensorMap& m);  // abi.cu
-
-inline int make_tmap_f16(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_b,
-                         const uint32_t* box, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B,
-                         const uint32_t* elem_strides = nullptr) {
-  TmapKey key;
-  memset(&key, 0, sizeof(key));  // padding bytes too: the key is compared and hashed as raw bytes
-  key.base = reinterpret_cast<uint64_t>(base);
-  key.rank = static_cast<uint32_t>(rank);
-  key.swizzle = static_cast<uint32_t>(swz);
-  for (int i = 0; i < rank; ++i) {
-    key.dims[i] = dims[i];
-    key.box[i] = box[i];
-    key.estr[i] = elem_strides ? elem_strides[i] : 1u;
-  }
-  for (int i = 0; i + 1 < rank; ++i) key.strides[i] = strides_b[i];
-  if (tmap_cache_lookup(key, m)) return AV2V_OK;
-  PFN_encodeTiled enc = get_encode_tiled();
-  if (!enc) return fail(AV2V_ECUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-  cuuint64_t gdim[5];
-  cuuint64_t gstr[5];
-  cuuint32_t bx[5];
-  cuuint32_t es[5];
-  for (int i = 0; i < rank; ++i) {
-    gdim[i] = dims[i];
-    bx[i] = box[i];
-    es[i] = elem_strides ? elem_strides[i] : 1u;
-  }
-  for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_b[i];
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, static_cast<cuuint32_t>(rank), const_cast<void*>(base), gdim,
-                   gstr, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    return fail(AV2V_ECUDA,
-                "cuTensorMapEncodeTiled failed (%d): rank %d dims [%llu %llu %llu %llu] box [%u %u %u %u] base %p",
-                (int)r, rank, (unsigned long long)dims[0], (unsigned long long)(rank > 1 ? dims[1] : 0),
-                (unsigned long long)(rank > 2 ? dims[2] : 0), (unsigned long long)(rank > 3 ? dims[3] : 0), box[0],
-                rank > 1 ? box[1] : 0, rank > 2 ? box[2] : 0, rank > 3 ? box[3] : 0, base);
-  }
-  tmap_cache_insert(key, *m);
-  return AV2V_OK;
-}
-
 int sm_count_cached();  // abi.cu
-
-// Kernel launch as thread-block clusters of `cluster_x` CTAs.
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, int cluster_x,
-                             Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  int na = 0;
-  if (cluster_x > 1) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = static_cast<unsigned>(cluster_x);
-    attr[na].val.clusterDim.y = 1;
-    attr[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = static_cast<unsigned>(na);
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-
-// attention2q_tcgen05.cu: two-query-tile attention (rows mode, n_v = 1); called by av2v_attn_pnp_f16 after validation
-int attn2q_launch(const ::av2v_attn_args* a, cudaStream_t stream);
 
 }  // namespace av2v

@@ -1,6 +1,6 @@
 """Tensor-level wrappers over the C ABI: PyTorch is used for device memory and streams only.
 
-Every function enqueues hand-written sm_100a kernels on the current CUDA stream; none has a PyTorch fallback.
+Every function enqueues hand-written sm_90a kernels on the current CUDA stream; none has a PyTorch fallback.
 Activations are channels-last (see include/anyv2v_b200.h).  ``launch_count()`` reports how many of OUR kernels
 were launched (bench.py's ``gpu_launches``).
 """
@@ -305,7 +305,7 @@ def attention(q, k, v, heads: int, seq: int, batch: int, out, scale: float = 0.1
 
 
 def temporal_attention_fused(x, wqkv, heads: int, F: int, HW: int, clips: int, out, scale: float = 0.125, n_v: int = 1):
-    """Temporal self-attention with the Q/K/V projection fused in (csrc/attention_tfused_tcgen05.cu; pnp_utils.py:247-334).
+    """Temporal self-attention with the Q/K/V projection fused in (csrc/attention_wgmma.cu; pnp_utils.py:247-334).
     x: frame-major tokens [clips*F*HW, Cx]; wqkv: [3*heads*64, Cx]; out: [clips*F*HW, heads*64].  n_v = 3: PnP-injected step,
     clips ordered [source | uncond | cond]; Q, K of every clip come from the source clip of the same index (pnp_utils.py:295-302)."""
     global _launches

@@ -1,4 +1,4 @@
-"""I2VGen-XL sampling loops, B200-native: ``invert`` and ``sample_with_pnp``.
+"""I2VGen-XL sampling loops, H100-native: ``invert`` and ``sample_with_pnp``.
 
 Drop-in for the two hot loops of the reference's ``I2VGenXLPipeline`` (i2vgen-xl/pipelines/pipeline_i2vgen_xl.py):
   invert            :1197-1439 (loop :1385-1433)
@@ -389,8 +389,8 @@ class I2VGenXLPipeline:
         st.graph_pool = torch.cuda.graph_pool_handle() if st.latents.is_cuda else None  # one activation pool for all of them
         # uncond and cond are the same latents + image latents -> they share the UNet prefix up to the first cross-attention
         # (I2VGenXLUNet.forward, shared_edit_prefix); the source branch is dropped after the last injection site that fires in
-        # the step (its prediction is discarded, pipeline :1160).  Both leave the result unchanged (measured +2.3 % / +0.9 % on
-        # the bench schedule, profiles/r02_probe.txt; `skip_dead_source_branch=False` runs the reference's full batch instead)
+        # the step (its prediction is discarded, pipeline :1160).  Both leave the result unchanged
+        # (`skip_dead_source_branch=False` runs the reference's full batch instead)
         st.shared_prefix = bool(skip_dead_source_branch)
         st.prune_source = bool(skip_dead_source_branch)
         return st

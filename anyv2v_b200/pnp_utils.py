@@ -9,9 +9,9 @@ Same four entry points, same call signatures and side effects (SURVEY 8b):
 ``up_blocks[1].resnets[1].forward`` and the ``attn1.processor`` of the 8 + 8 PnP sites, and re-registration is
 idempotent — exactly as in the reference.  What the replaced code *does* is different: on a scheduled timestep
   * the resnet computes norm1/conv1/norm2/conv2 for the SOURCE frames only and the conv2 epilogue stores the tile to
-    the three branch slots (fused conv + residual-copy, anyv2v_b200/csrc/gemm_tcgen05.cu);
-  * the attention projects q,k for the source third only and one tcgen05 kernel applies the shared probabilities
-    to [V_src | V_uncond | V_cond] (anyv2v_b200/csrc/attention_tcgen05.cu).
+    the three branch slots (fused conv + residual-copy, anyv2v_b200/csrc/gemm_wgmma.cu);
+  * the attention projects q,k for the source third only and one wgmma kernel applies the shared probabilities
+    to [V_src | V_uncond | V_cond] (anyv2v_b200/csrc/attention_wgmma.cu).
 Outputs equal the reference's (which computes everything three times and then overwrites two thirds).
 The membership test ``t in schedule or t == 1000`` is evaluated on the host from a Python set — no device sync.
 """

@@ -4,7 +4,7 @@ Same CLI (``--template_config``, ``--configs_json``; reference :186-192), same Y
 semantics (template merged with each JSON entry, ``"active": false`` skips; :74-81), same ``init_pnp`` arithmetic
 (:35-48), same ``ddim_latents_{t}.pt`` inputs and the same output directory naming (:154-168).
 What changes: clips are sharded one-per-GPU when launched under torchrun (the reference loops over them on one
-device, :74) and the models are this package's B200 UNet / VAE plus the ``transformers`` CLIP towers.  The runner consumes
+device, :74) and the models are this package's UNet / VAE plus the ``transformers`` CLIP towers.  The runner consumes
 the REAL inputs like the reference (:95-150): source frames ``{video_dir}/{video_name}/%05d.png`` (mp4 fallback), the edited
 first frame, the prompts; it decodes the result with the VAE and writes ``video.mp4`` / ``video.gif`` / ``video_%05d.png``
 (:169-183) plus ``edited_latents.pt``.  Weights: ``model_name`` may name a local diffusers-layout checkpoint directory

@@ -1,4 +1,4 @@
-"""I2VGen-XL 3-D UNet, B200-native forward.
+"""I2VGen-XL 3-D UNet, H100-native (sm_90a) forward.
 
 The module / parameter names are those of diffusers==0.26.3 ``I2VGenXLUNet`` (the model the reference drives at
 i2vgen-xl/pipelines/pipeline_i2vgen_xl.py:1146-1155 and whose sub-modules i2vgen-xl/pnp_utils.py patches), so that a
@@ -9,8 +9,8 @@ What differs is everything underneath:
   * activations are channels-last for the whole network; a frame batch is [B*F, H, W, C] and the same memory viewed
     as [B, F*H*W, C] IS the frame-major token matrix of the temporal layers — the reference's
     [B,C,F,h,w] <-> [B*F,C,h,w] <-> [B*hw,F,C] permute/reshape copies do not exist;
-  * GroupNorm+SiLU, every 3x3 conv (implicit GEMM, TMA taps), every temporal (3,1,1) conv, every Linear and all
-    self-attention run on the hand-written sm_100a kernels of anyv2v_b200.ops;
+  * GroupNorm+SiLU, every 3x3 conv (implicit GEMM, cp.async-gathered taps), every temporal (3,1,1) conv, every Linear and all
+    self-attention run on the hand-written sm_90a kernels of anyv2v_b200.ops;
   * LayerNorm and the GEGLU gate (fused into the FF GEMM's epilogue) are hand-written too; the few layers SURVEY 8(f)
     leaves as "next" (stride-2 / tiny stem convs, 145-token cross-attention SDPA, nearest up-sampling, skip concat)
     are library calls collected in anyv2v_b200.next_rows.
@@ -68,7 +68,7 @@ class Linear(nn.Linear):
 
 
 class Conv3x3(nn.Conv2d):
-    """3x3 / pad 1 convolution run as an implicit GEMM on tcgen05 (ops.conv3x3), stride 1 or 2 (Downsample2D).
+    """3x3 / pad 1 convolution run as an implicit GEMM on wgmma (ops.conv3x3), stride 1 or 2 (Downsample2D).
 
     Widths the tensor-core tiles do not cover are padded in the PACKED weight only (the parameter keeps its diffusers shape):
     Cin not a multiple of 64 (conv_in: 8 input channels) -> every tap's K block is zero-padded to 64 and the activation's missing
@@ -121,7 +121,7 @@ class GroupNorm(nn.GroupNorm):
 
 # ------------------------------------------------------------------------------------------------ attention
 class AttnProcessor:
-    """B200 attention processor with the diffusers protocol (pnp_utils.py:142-150).
+    """Attention processor of this package with the diffusers protocol (pnp_utils.py:142-150).
 
     hidden_states is either the protocol's [batch, seq, C] tensor, or — fast path used by this package's temporal
     transformers — a 4-D frame-major view [B, HW, F, C] (strides (F*HW*C, C, HW*C, 1)) so that no transposed copy of
@@ -265,7 +265,7 @@ class _GEGLU(nn.Module):
 
     def packed(self):
         """(weight, bias) with the h / gate halves interleaved in blocks of 32 rows: the layout of the fused GEGLU
-        epilogue (csrc/gemm_tcgen05.cu), which stores h * gelu_erf(gate) and never materialises the [rows, 8C] tensor."""
+        epilogue (csrc/gemm_wgmma.cu), which stores h * gelu_erf(gate) and never materialises the [rows, 8C] tensor."""
         w = self.proj.weight
         key = (w.data_ptr(), w._version, self.proj.bias.data_ptr(), self.proj.bias._version)
         if self._packed._key != key:

@@ -1,12 +1,12 @@
-"""AutoencoderKL (the KL-f8 VAE of `ali-vilab/i2vgen-xl`) on the hand-written sm_100a kernels — SURVEY §8f row 4: the
+"""AutoencoderKL (the KL-f8 VAE of `ali-vilab/i2vgen-xl`) on the hand-written sm_90a kernels — SURVEY §8f row 4: the
 steps either side of the sampling loops, `encode_vae_video` (i2vgen-xl/pipelines/pipeline_i2vgen_xl.py:565-592) and
 `decode_latents` (:443-463).
 
 Module / parameter names are diffusers' (`encoder.down_blocks.0.resnets.0.norm1.weight`, `decoder.mid_block.attentions.0.to_q…`,
 `quant_conv`, `post_quant_conv`), so a real `diffusion_pytorch_model` state_dict loads unchanged.  Activations are
 channels-last fp16 end to end; every 3x3 convolution with Cin % 64 == 0 (all but `conv_in`), every GroupNorm(+SiLU),
-the 1x1 shortcuts and the attention projections run on `anyv2v_b200.ops` (tcgen05 implicit GEMM, fused bias/residual
-epilogue; image widths above 128 are tiled as 128-pixel row segments).  Left on library calls for now
+the 1x1 shortcuts and the attention projections run on `anyv2v_b200.ops` (wgmma implicit GEMM, fused bias/residual
+epilogue).  Left on library calls for now
 (`next_rows`): `conv_in` (3 -> 128), the convolutions that end in 3 / 8 / 4 channels, the stride-2 down-sampling
 convolutions, and the single-head 512-wide mid-block attention core (head_dim 512 is outside the d = 64 kernel).
 There is no CPU path.

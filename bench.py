@@ -1,7 +1,8 @@
-"""Benchmark of the AnyV2V hot path on B200: denoising-steps/sec of I2VGen-XL DDIM inversion + PnP edit.
+"""Benchmark of the AnyV2V hot path on H100: denoising-steps/sec of I2VGen-XL DDIM inversion + PnP edit.
 
   python bench.py --gpus N --steps K --warmup W            # this package (CUDA kernels through the C ABI)
   python bench.py --impl reference --gpus N --steps K ...   # the reference path's CPU port (oracle) on the host cores
+  python bench.py --gpus 1 --steps K --dump-outputs DIR     # + the last timed step's outputs as DIR/<name>.npy (float32)
 
 Workload (BASELINE.json configs[1], the configuration the metric is quoted on): one 16-frame 512x512 clip
 (latents [1,4,16,64,64]), full-size random-init I2VGen-XL UNet (1.42 B params, fp16), 50-step schedules, guidance 9.0,
@@ -55,11 +56,12 @@ def measured_peaks():
             d = json.load(fh)
         return dict(source="measured (MEASURED_PEAKS.json)", hbm_gbs=d["hbm_gbs"], tflops_burst=d["bf16_tflops"],
                     tflops_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]))
-    return dict(source="fallback (B200_PROFILING.md)", hbm_gbs=6650.0, tflops_burst=1590.0, tflops_sustained=1400.0)
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth, dense FP16 tensor rate
+    return dict(source="H100 SXM data sheet", hbm_gbs=3350.0, tflops_burst=989.0, tflops_sustained=989.0)
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -163,6 +165,7 @@ def run_ours(args):
         return inv_sched, st_inv, st_edit
 
     launches_per_step = {}
+    last_out = {}  # what the most recent invert_step / edit_step returned
 
     def run_steps(inv_sched, st_inv, st_edit, i0_inv, n_inv, i0_edit, n_edit, d2h_result=None):
         pipe.scheduler = inv_sched
@@ -170,6 +173,7 @@ def run_ours(args):
             c0 = ops.launch_count()
             x = pipe.invert_step(st_inv, i)
             launches_per_step.setdefault("inv", ops.launch_count() - c0)  # first (eager) pass = launches per step
+            last_out["inversion_latents"] = x
             if d2h_result is not None:
                 d2h_result.copy_(x, non_blocking=True)
         pipe.scheduler = edit_sched
@@ -177,6 +181,7 @@ def run_ours(args):
             c0 = ops.launch_count()
             x = pipe.edit_step(st_edit, i)
             launches_per_step.setdefault("edit", ops.launch_count() - c0)
+            last_out["edit_latents"] = x
             if d2h_result is not None:
                 d2h_result.copy_(x, non_blocking=True)
 
@@ -211,6 +216,8 @@ def run_ours(args):
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1)
+    # the timed path's results of its last inversion and last edit step, copied before any later pass overwrites them
+    dumped = {k: v.float().cpu().numpy() for k, v in last_out.items()}
     graphs = pipe.use_cuda_graphs
     # kernels launched per replayed step are the ones recorded at capture time
     launches = ops.launch_count() - l0
@@ -281,7 +288,7 @@ def run_ours(args):
                    "parity": "DDIM / CFG step bit-exact vs the oracle; kernels vs fp32 restatements at rtol 1e-3 + 1e-3..2e-3 x max|ref| "
                              "(one fp16 rounding is 4.9e-4 relative; north_star's literal atol 1e-4 is below fp16 resolution for |x| > 0.2); "
                              "full-width (1.42 B params) hooked UNet steps as close to the fp32 oracle as torch fp16 is (x3) — tests/",
-                   "l2": "per-step working set (2.84 GB fp16 weights + activations) >> 126 MB L2; no explicit flush",
+                   "l2": "per-step working set (2.84 GB fp16 weights + activations) >> 50 MB L2; no explicit flush",
                    "ms_per_inversion_step": round(ms_inv, 3), "ms_per_edit_step": round(ms_edit, 3),
                    "effective_tflops_reference_flops": round((k_inv * TFLOP_INV + k_edit * TFLOP_EDIT) * (F / 16) / (ms_max * 1e-3), 1),
                    "outputs_finite": finite, "model_build_s": round(build_s, 1)},
@@ -301,7 +308,18 @@ def run_ours(args):
         out["metric"] = METRIC.replace("16f", f"{F}f")
     if not args.no_cpu_baseline and world >= 1:
         out["cpu_baseline"] = cpu_baseline(budget_s=args.cpu_budget)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, dumped)
     print(json.dumps(out), flush=True)
+
+
+def dump_outputs(directory, arrays):
+    """DIR/<name>.npy per output; the inputs are seeded, so two builds run with the same arguments compare array for array"""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    assert sum(a.nbytes for a in arrays.values()) <= 64 << 20
+    for name, a in arrays.items():
+        np.save(os.path.join(directory, f"{name}.npy"), a)
 
 
 def attention_roofline(ops, dev):
@@ -328,37 +346,12 @@ def attention_roofline(ops, dev):
     dur = e0.elapsed_time(e1) / iters * 1e-3
     flops = 2.0 * batch * heads * seq * seq * 64 * (1 + 3)
     achieved = flops / dur / 1e12
-    return {"kernel": "attn_pnp_kernel<3> (spatial PnP self-attention, up_blocks[3] site: 16 src frames x 5 heads x 4096 tokens, shared P)",
+    return {"kernel": "attn_kernel<3> (spatial PnP self-attention, up_blocks[3] site: 16 src frames x 5 heads x 4096 tokens, shared P)",
             "bound": "tensor", "achieved": round(achieved, 1), "peak": peaks["tflops_burst"], "unit": "TFLOP/s",
             "frac": round(achieved / peaks["tflops_burst"], 4),
-            # dram__bytes_read.sum + dram__bytes_write.sum per launch of this geometry, read at run time from the committed
-            # `ncu --set full` capture (null when the file is absent); algorithmic minimum 0.34 GB (q, k + 3 v + 3 o)
-            **ncu_traffic(("r02_attn3.ncu.csv", "r01_prof_attn3_v9.ncu.csv"), "attn_pnp_kernel"),
             "peak_source": peaks["source"] + ", burst (kernel timed alone, back-to-back launches, q/k/v 0.25 GB > L2)",
             "us_per_launch": round(dur * 1e6, 1),
             "algorithmic_flops_per_launch": flops}
-
-
-def ncu_traffic(csv_names, kernel_substr):
-    """{"traffic": dram__bytes_read.sum + dram__bytes_write.sum of `kernel_substr`'s launch in the first committed ncu summary of
-    `csv_names` under profiles/ (`metric,unit,value` rows written by tools/ncu_extract.py from an `ncu --set full` report),
-    "traffic_unit": where it came from}; traffic = None when no capture is committed — never a constant typed into this file."""
-    import csv
-    scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    for name in csv_names:
-        path = os.path.join(ROOT, "profiles", name)
-        if not os.path.exists(path):
-            continue
-        try:
-            with open(path, newline="") as fh:
-                rows = {r[0]: r for r in csv.reader(fh) if len(r) >= 3}
-            if kernel_substr not in rows["Kernel Name"][2]:
-                continue
-            tot = sum(float(rows[m][2].replace(",", "")) * scale[rows[m][1]] for m in ("dram__bytes_read.sum", "dram__bytes_write.sum"))
-            return {"traffic": tot, "traffic_unit": f"bytes/launch (ncu dram__bytes_read.sum + dram__bytes_write.sum, profiles/{name})"}
-        except (KeyError, ValueError, IndexError, OSError):
-            continue
-    return {"traffic": None, "traffic_unit": "no committed ncu capture found under profiles/"}
 
 
 def _time_us(fn, iters=20, warm=3):
@@ -388,12 +381,11 @@ def temporal_attention_roofline(ops, dev):
     us = _time_us(lambda: ops.temporal_attention_fused(x, w, heads, frames, hw, clips, out, n_v=3))
     nbytes = 2.0 * rows * C * 2
     gbs = nbytes / us / 1e3
-    return {"kernel": "tattn_fused2_kernel, injected (temporal PnP self-attention, up_blocks[3] site: [src|uncond|cond] x 16 f x 4096 px, C 320)",
+    return {"kernel": "tattn_fused_kernel<3>, injected (temporal PnP self-attention, up_blocks[3] site: [src|uncond|cond] x 16 f x 4096 px, C 320)",
             "bound": "hbm", "achieved": round(gbs, 1), "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": round(gbs / peaks["hbm_gbs"], 4),
-            **ncu_traffic(("r02_tattn_fused.ncu.csv",), "tattn_fused"), "us_per_launch": round(us, 1),
-            "algorithmic_bytes_per_launch": nbytes, "peak_source": peaks["source"],
-            "note": "projection FLOPs 2*rows*320*960 + 3x re-projected q,k (injected variant) make this kernel L2->SM-fabric bound, "
-                    "not HBM-bound, today: see DESIGN.md"}
+            "us_per_launch": round(us, 1), "algorithmic_bytes_per_launch": nbytes, "peak_source": peaks["source"],
+            "note": "the in-kernel projection (2*rows*320*960 FLOPs, per head re-reading the tokens from L2) is not counted in the "
+                    "HBM bound"}
 
 
 def groupnorm_roofline(ops, dev):
@@ -408,7 +400,7 @@ def groupnorm_roofline(ops, dev):
     gbs = nbytes / us / 1e3
     return {"kernel": "gn_persistent_kernel (GroupNorm+SiLU [3, 65536, 320], TemporalConvLayer norms of the 64x64 level)", "bound": "hbm",
             "achieved": round(gbs, 1), "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": round(gbs / peaks["hbm_gbs"], 4),
-            **ncu_traffic(("r02_groupnorm.ncu.csv",), "gn_persistent_kernel"), "us_per_launch": round(us, 1),
+            "us_per_launch": round(us, 1),
             "algorithmic_bytes_per_launch": nbytes, "peak_source": peaks["source"]}
 
 
@@ -421,8 +413,8 @@ def gemm_rooflines(ops, dev):
     out = []
     M, K = 196608, 320
     a = torch.randn(M, K, device=dev).half()
-    for name, N, geglu, csv_name in (("linear 196608x960x320 (+bias; q|k|v projection of the 64x64 level)", 960, False, "r02_gemm_lin960.ncu.csv"),
-                                     ("linear+GEGLU 196608x2560x320 (feed-forward of the 64x64 level, 1280 output columns)", 2560, True, "r02_gemm_geglu.ncu.csv")):
+    for name, N, geglu in (("linear 196608x960x320 (+bias; q|k|v projection of the 64x64 level)", 960, False),
+                           ("linear+GEGLU 196608x2560x320 (feed-forward of the 64x64 level, 1280 output columns)", 2560, True)):
         w = (torch.randn(N, K, device=dev) / 18).half()
         b = torch.randn(N, device=dev).half()
         if geglu:
@@ -434,11 +426,11 @@ def gemm_rooflines(ops, dev):
         tf, gbs = flops / us / 1e6, nbytes / us / 1e3
         t_tensor, t_hbm = flops / (peaks["tflops_sustained"] * 1e6), nbytes / (peaks["hbm_gbs"] * 1e3)
         bound = "tensor" if t_tensor >= t_hbm else "hbm"
-        out.append({"kernel": f"gemm_tcgen05_kernel ({name})", "bound": bound,
+        out.append({"kernel": f"gemm_wgmma_kernel ({name})", "bound": bound,
                     "achieved": round(tf if bound == "tensor" else gbs, 1),
                     "peak": peaks["tflops_sustained"] if bound == "tensor" else peaks["hbm_gbs"],
                     "unit": "TFLOP/s" if bound == "tensor" else "GB/s",
-                    "frac": round(max(t_tensor, t_hbm) / us, 4), **ncu_traffic((csv_name,), "gemm_tcgen05_kernel"),
+                    "frac": round(max(t_tensor, t_hbm) / us, 4),
                     "us_per_launch": round(us, 1), "algorithmic_flops_per_launch": flops, "algorithmic_bytes_per_launch": nbytes,
                     "tensor_bound_us": round(t_tensor, 1), "hbm_bound_us": round(t_hbm, 1),
                     "peak_source": peaks["source"] + ", sustained (the kernel runs inside a long power-capped step)"})
@@ -680,11 +672,17 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=4)
     ap.add_argument("--impl", type=str, default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="after the timed steps, write the latents the last timed inversion step and the last timed edit step "
+                         "returned as DIR/inversion_latents.npy and DIR/edit_latents.npy (float32); the timed steps are the first "
+                         "ceil(K/2) inversion and floor(K/2) edit steps, so --steps 1 times no edit step and writes no edit_latents")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--frames", type=int, default=16, help="frames per clip: 16 (BASELINE configs[1], default) or 128 (configs[4])")
     ap.add_argument("--cpu-budget", type=float, default=40.0)
     ap.add_argument("--ref-budget", type=float, default=150.0)
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs dumps the GPU path's outputs; it is not available with --impl reference")
     global F
     F = args.frames
     if args.warmup < 4:

@@ -1,5 +1,5 @@
 /*
- * anyv2v_b200 — C ABI of the B200-native AnyV2V hot path (DDIM inversion + PnP edit over the I2VGen-XL UNet).
+ * anyv2v_b200 — C ABI of the H100-native (sm_90a) AnyV2V hot path (DDIM inversion + PnP edit over the I2VGen-XL UNet).
  *
  * The reference (TIGER-AI-Lab/AnyV2V) is 100 % Python and has no FFI of its own; every kernel it runs is a
  * library call inside PyTorch/diffusers.  This header is therefore the NEW boundary that sits *under* the
@@ -35,7 +35,8 @@ enum {
 
 int av2v_abi_version(void);
 const char* av2v_last_error(void); /* thread-local, valid until the next failing call on this thread */
-/* device properties the host side sizes its launches with; returns AV2V_ECUDA when no sm_100 device is current */
+/* device properties the host side sizes its launches with; returns AV2V_ECUDA when no device is current and
+   AV2V_ENOSUP when the current device is not sm_90 (compute capability 9.0) */
 int av2v_device_info(int* sm_count, int* cc_major, int* cc_minor);
 
 /* ------------------------------------------------------------------------------------------------------------
@@ -91,12 +92,12 @@ typedef struct {
 int av2v_groupnorm_silu_f16(const av2v_groupnorm_args* a, av2v_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------
- * tcgen05 GEMM core:  out[slot][m, n] = sum_k A[m, k] * Wt[n, k] + bias[n] + rowbias[m / rows_per_rowbias, n]
+ * wgmma GEMM core:  out[slot][m, n] = sum_k A[m, k] * Wt[n, k] + bias[n] + rowbias[m / rows_per_rowbias, n]
  *                                        + residual[slot][m, n]
- * A operand modes (all fed by TMA straight from the channels-last activation, no im2col buffer):
+ * A operand modes (all gathered by cp.async straight from the channels-last activation, no im2col buffer):
  *   AV2V_A_LINEAR : A is [M, K] row-major (lda elements)                      -> nn.Linear / 1x1 conv
  *   AV2V_A_CONV3X3: A is [NF, H, W, Cin]; K = 9*Cin, zero padding 1            -> Conv2d 3x3 (pnp_utils.py:78,107);
- *                   stride 2 (Downsample2D) samples the taps with TMA element strides; a_channels < Cin reads the
+ *                   stride 2 (Downsample2D) samples every second input pixel; a_channels < Cin reads the
  *                   missing channels as zeros (conv_in: 8 channels in a 64-wide K block, weights zero-padded)
  *   AV2V_A_TCONV3 : A is [B, F*HW, Cin]; K = 3*Cin, zero padding over frames   -> Conv3d (3,1,1) of TemporalConvLayer
  * LINEAR with a2 != NULL: the logical A is [a | a2] along K (columns [0, k_split) from a, [k_split, K) from a2) — the
@@ -152,7 +153,7 @@ typedef struct {
 int av2v_layernorm_f16(const av2v_layernorm_args* a, av2v_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------
- * K1-K3  PnP self-attention core (head_dim 64): softmax(Q K^T * scale) V on tcgen05, with the PnP Q/K injection
+ * K1-K3  PnP self-attention core (head_dim 64): softmax(Q K^T * scale) V on wgmma, with the PnP Q/K injection
  * folded in.  Replaces pnp_utils.py:189-210 (spatial) and :295-316 (temporal): F.scaled_dot_product_attention
  * plus the slice-assign injection copies.
  *   - q, k, v are token matrices with arbitrary row stride (so a fused [rows, 3C] QKV buffer works), head h
@@ -201,15 +202,6 @@ typedef struct {
   int32_t n_v;                 /* 1 | 3 */
 } av2v_tattn_fused_args;
 int av2v_tattn_fused_f16(const av2v_tattn_fused_args* a, av2v_stream_t stream);
-
-/* ------------------------------------------------------------------ diagnostics (bring-up; not part of the drop-in path)
- * Role timers of CTA 0 of the last av2v_gemm_f16 launch made with the environment variable AV2V_GEMM_DEBUG=8:
- * out16[0..4] = producer wait-empty, producer total, MMA wait-tmem-empty, MMA wait-full, MMA total (SM cycles).
- * Synchronises the device. */
-int av2v_gemm_debug_timers(unsigned long long* out16);
-/* TMA descriptor cache (CUtensorMaps keyed by base pointer + shape + strides + box + swizzle, mutex-guarded, bounded): lookups
- * that hit / missed since the library was loaded and the number of cached descriptors.  Any pointer may be NULL. */
-int av2v_tmap_cache_stats(long long* hits, long long* misses, int* entries);
 
 #ifdef __cplusplus
 }

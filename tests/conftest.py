@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
     # the fp32 oracle must be fp32 on the GPU box too: TF32 (10-bit mantissa, cuDNN's default for convolutions) would make
     # the "fp32 reference" no more precise than the fp16 kernels it judges
     import torch

@@ -1,4 +1,4 @@
-"""GPU parity tests, kernel level: each hand-written sm_100a kernel (called through the C ABI) against an fp32
+"""GPU parity tests, kernel level: each hand-written sm_90a kernel (called through the C ABI) against an fp32
 PyTorch restatement of the same op on identical fp16 inputs; the DDIM step against the oracle bit for bit."""
 import pytest
 import torch
@@ -21,7 +21,7 @@ def test_native_library_is_loaded(ops):
     lib = _lib.lib()
     sm, maj, mnr = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
     _lib.check(lib.av2v_device_info(ctypes.byref(sm), ctypes.byref(maj), ctypes.byref(mnr)), "device_info")
-    assert maj.value == 10 and sm.value >= 100
+    assert (maj.value, mnr.value) == (9, 0) and sm.value >= 100
 
 
 @pytest.mark.parametrize("n", [8, 4 * 16 * 64 * 64, 1001])
@@ -250,12 +250,11 @@ def _ref_attn(q, k, v, heads, scale=0.125):
 
 @pytest.mark.parametrize("case", [(1, 1, 128, 1.0), (2, 2, 256, 1.0), (2, 2, 1024, 3.0), (1, 1, 200, 1.0), (3, 2, 384, 1.0),
                                   (1, 2, 880, 2.0), (4, 5, 4096, 1.0), (1, 1, 64, 1.0), (2, 1, 300, 6.0),
-                                  # >= 16 key tiles: two threads per query row (attn2q_split_kernel): ragged tails, odd tile counts
+                                  # long key loops: ragged tails, odd tile counts
                                   (2, 1, 2048, 1.0), (1, 2, 2100, 3.0), (1, 1, 2300, 6.0), (1, 3, 2176 + 64, 2.0)])
 def test_attention_two_query_tiles_rows(ops, case):
-    """plain (n_v = 1) rows-mode attention = the two-query-tile kernels (csrc/attention2q_tcgen05.cu; one / two threads per
-    query row below / from 16 key tiles): odd tile counts, ragged tails, large-magnitude scores (rescale path), against an
-    fp32 restatement"""
+    """plain (n_v = 1) rows-mode attention, 128 queries per CTA (csrc/attention_wgmma.cu): odd tile counts, ragged tails,
+    large-magnitude scores (rescale path), against an fp32 restatement"""
     batch, heads, seq, mag = case
     torch.manual_seed(6)
     C = heads * 64
@@ -269,8 +268,8 @@ def test_attention_two_query_tiles_rows(ops, case):
 
 @pytest.mark.parametrize("seq", [1024, 3072])
 def test_attention_two_query_tiles_rescale_path(ops, seq):
-    """keys whose scores grow along the sequence force the running max up by > 2^8 several times: O is rescaled in TMEM
-    (3072 keys: the two-threads-per-row kernel, where each half rescales 32 of O's 64 columns)"""
+    """keys whose scores grow along the sequence force the running max up again and again: O and the row sum are rescaled in
+    registers on every raise"""
     torch.manual_seed(9)
     batch, heads = 1, 1
     q = torch.randn(batch * seq, 64, device=dev).half()
@@ -286,10 +285,10 @@ def test_attention_two_query_tiles_rescale_path(ops, seq):
 @pytest.mark.parametrize("nv", [1, 3])
 @pytest.mark.parametrize("case", [(3, 5, 16, 4096, 320), (1, 8, 16, 4096, 512), (2, 10, 16, 1024, 640), (3, 20, 16, 256, 1280), (1, 2, 8, 256, 128),
                                   (1, 1, 128, 16, 64), (2, 2, 4, 16, 128), (1, 2, 16, 100, 128), (1, 1, 32, 7, 64),
-                                  # two-items-in-flight kernel (>= 2 items per CTA, Cx <= 640): ragged pixel tiles, 2 and 5 k-blocks, 8 heads x 320
+                                  # ragged pixel tiles, 2 and 5 k-blocks, 8 heads x 320
                                   (2, 5, 16, 1001, 320), (4, 2, 16, 2048, 128), (1, 8, 16, 4096, 320), (1, 5, 128, 160, 320), (2, 3, 8, 1024, 192)])
 def test_temporal_attention_fused(ops, case, nv):
-    """Q/K/V projection + temporal attention in ONE launch (csrc/attention_tfused_tcgen05.cu, pnp_utils.py:247-334) vs the
+    """Q/K/V projection + temporal attention in ONE launch (csrc/attention_wgmma.cu, pnp_utils.py:247-334) vs the
     two-kernel path (same rounding points: Q, K, V to fp16, P to fp16) and vs an fp32 restatement.  nv = 3: PnP-injected
     (clips = [source | uncond | cond] x `clips` each; Q, K of every branch from the source clip, pnp_utils.py:295-302)."""
     clips, heads, F, HW, Cx = case
@@ -363,32 +362,6 @@ def test_groupnorm_sample_larger_than_l2(ops):
     ref = torch.nn.functional.silu(torch.nn.functional.group_norm(x.float().transpose(1, 2), 32, g.float(), b.float(), 1e-5)
                                    .transpose(1, 2).half().float())
     assert_fp16_close(got, ref, "groupnorm 128-frame clip", atol_frac=2e-3)
-
-
-def test_tensor_map_descriptors_are_cached(ops):
-    """SURVEY 8b: the library keeps nothing persistent except CUtensorMaps keyed by (pointer, shape): a repeated launch on the
-    same buffers must be served from the cache (no cuTensorMapEncodeTiled call), a new shape must miss"""
-    import ctypes
-    from anyv2v_b200 import _lib
-    lib = _lib.lib()
-
-    def stats():
-        h, m, n = ctypes.c_longlong(), ctypes.c_longlong(), ctypes.c_int()
-        _lib.check(lib.av2v_tmap_cache_stats(ctypes.byref(h), ctypes.byref(m), ctypes.byref(n)), "tmap_cache_stats")
-        return h.value, m.value, n.value
-
-    a = torch.randn(512, 320, device=dev).half()
-    w = torch.randn(640, 320, device=dev).half()
-    out = torch.empty(512, 640, device=dev, dtype=torch.float16)
-    ops.linear(a, w, out=out)
-    h0, m0, n0 = stats()
-    first = out.clone()
-    ops.linear(a, w, out=out)
-    h1, m1, n1 = stats()
-    assert m1 == m0 and n1 == n0 and h1 >= h0 + 3 and torch.equal(out, first)  # A, W and the output descriptor: all hits
-    ops.linear(a[:256], w, out=out[:256])
-    h2, m2, n2 = stats()
-    assert m2 > m1 and n2 > n1
 
 
 @pytest.mark.parametrize("geo", [(48, 64, 64, 320, 320), (6, 32, 32, 640, 640), (4, 16, 16, 1280, 1280), (3, 8, 8, 128, 64), (5, 4, 4, 64, 128), (2, 2, 2, 64, 64)])

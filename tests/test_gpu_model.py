@@ -1,4 +1,4 @@
-"""GPU parity tests, model level: the B200 UNet + hooks + loops against the oracle (run on the same GPU with torch
+"""GPU parity tests, model level: the sm_90a UNet + hooks + loops against the oracle (run on the same GPU with torch
 ops, fp32 and fp16) on identical seeded weights / latents."""
 from types import SimpleNamespace
 

@@ -42,10 +42,10 @@ def test_ops_refuse_cpu_tensors_loudly():
         ops.groupnorm(torch.zeros(1, 4, 32, dtype=torch.float16), torch.ones(32).half(), torch.zeros(32).half(), 32, 1e-5, True)
 
 
-REF_CFG = "/root/reference/i2vgen-xl/configs"
+# the reference's own config templates and group configs (i2vgen-xl/configs/), stored as test data
+REF_CFG = os.path.join(ROOT, "tests", "golden", "reference_configs")
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_CFG), reason="reference configs only exist in the build container")
 def test_config_api_on_the_reference_templates():
     from anyv2v_b200.config import OmegaConf
     t = OmegaConf.load(f"{REF_CFG}/group_pnp_edit/template.yaml")
@@ -257,21 +257,7 @@ def test_bench_cpu_arm_thread_budget_respects_the_cgroup_quota(monkeypatch):
         pass
 
 
-def test_bench_roofline_traffic_comes_from_the_committed_ncu_extracts():
-    """bench.py never types DRAM traffic in: `roofline.traffic` is read from the `metric,unit,value` extracts of `ncu --set full`
-    reports committed under profiles/ (tools/ncu_extract.py); a missing capture or a capture of another kernel gives None."""
-    import bench
-    for csv_name, kernel in (("r02_attn3.ncu.csv", "attn_pnp_kernel"), ("r02_tattn_fused.ncu.csv", "tattn_fused"),
-                             ("r02_groupnorm.ncu.csv", "gn_persistent_kernel"), ("r02_gemm_lin960.ncu.csv", "gemm_tcgen05_kernel"),
-                             ("r02_gemm_geglu.ncu.csv", "gemm_tcgen05_kernel")):
-        got = bench.ncu_traffic((csv_name,), kernel)
-        assert got["traffic"] is not None and 1e7 < got["traffic"] < 5e9, (csv_name, got)
-        assert csv_name in got["traffic_unit"]
-    assert bench.ncu_traffic(("r02_groupnorm.ncu.csv",), "attn_pnp_kernel")["traffic"] is None   # capture of another kernel
-    assert bench.ncu_traffic(("no_such_file.csv",), "gemm_tcgen05_kernel")["traffic"] is None
-
-
-@torch.no_grad()
+@torch.no_grad()  # the pipeline runs its VAE brackets without autograd; do not depend on an earlier test having disabled it
 def test_pipeline_vae_brackets_and_tensor2vid_on_cpu():
     """Host logic of the steps either side of the loops (pipeline_i2vgen_xl.py:79-97, :443-463, :565-592): the pipeline
     delegates to whatever module speaks diffusers' VAE protocol — here the oracle VAE on the CPU — and `tensor2vid`
@@ -303,74 +289,88 @@ def test_pipeline_vae_brackets_and_tensor2vid_on_cpu():
 
 
 def test_attn2q_barrier_protocol_model():
-    """tools/protocol_sim.py restates the warp roles of csrc/attention2q_tcgen05.cu (same waits / arrives / commits, same
-    parity expressions) and runs them under randomised latencies: no deadlock, no buffer hazard."""
+    """tools/kernel_models.py restates the K / V double buffer of attn_kernel (csrc/attention_wgmma.cu: prefetch of tile kt + 1,
+    wait_group, fence + __syncthreads, both warpgroups compute, trailing __syncthreads) as a discrete-event model: no tile is
+    read before it landed and no buffer is overwritten while a warpgroup still reads it, under randomised latencies — and the
+    model does catch the hazard when the trailing barrier is dropped."""
     import random
-    from tools import protocol_sim
-    rng = random.Random(7)
-    for items, n_kv, stages in ((1, 1, 4), (2, 2, 4), (3, 8, 4), (2, 32, 4), (5, 3, 2), (3, 7, 3)):
-        for _ in range(6):
-            protocol_sim.simulate_attn2q(random.Random(rng.getrandbits(32)), items, n_kv, stages)
-    # attn2q_split_kernel: two warps per lane quarter and query tile, row maximum exchanged through double-buffered slots + a named barrier
-    for items, n_kv, stages in ((1, 16, 4), (2, 32, 4), (3, 17, 3), (2, 1, 4)):
-        for _ in range(4):
-            protocol_sim.simulate_attn2q(random.Random(rng.getrandbits(32)), items, n_kv, stages, split=True)
+    from tools import kernel_models as km
+    src = open(os.path.join(ROOT, "anyv2v_b200", "csrc", "attention_wgmma.cu")).read()
+    assert "every warpgroup is done with this buffer before the next prefetch overwrites it" in src
+    rng = random.Random(5)
+    for n in (1, 2, 3, 8, 64):
+        for _ in range(20):
+            km.simulate_double_buffer(random.Random(rng.getrandbits(32)), n)
     caught = 0
-    for _ in range(10):  # negative control: one exchange buffer instead of two -> a late read sees the partner's NEXT tile
+    for _ in range(20):
         try:
-            protocol_sim.simulate_attn2q(random.Random(rng.getrandbits(32)), 2, 24, 4, split=True, single_xchg_buffer=True)
+            km.simulate_double_buffer(random.Random(rng.getrandbits(32)), 16, trailing_barrier=False)
         except AssertionError:
             caught += 1
-    assert caught == 10
+    assert caught >= 15
 
 
 def test_fused_temporal_attention_barrier_protocol_model():
-    """csrc/attention_tfused_tcgen05.cu: projection ring -> convert -> S -> softmax -> PV with the next item's projection
-    issued under the current softmax"""
+    """tattn_fused_kernel: the projection ring (project(): the same double buffer over Cx / 64 K blocks) and the hand-off of
+    the Q / K / V tiles from the projection to the attention (each warpgroup stores its own 64 rows, then reads key rows of
+    both halves: fence + __syncthreads in between) — no hazard under randomised latencies, and a missing hand-off barrier is
+    caught."""
     import random
-    from tools import protocol_sim
-    rng = random.Random(5)
-    for items, num_kb, stages in ((1, 5, 4), (3, 5, 4), (6, 20, 4), (4, 1, 2), (5, 8, 3)):
-        for _ in range(6):
-            protocol_sim.simulate_tfused(random.Random(rng.getrandbits(32)), items, num_kb, stages)
+    from tools import kernel_models as km
+    rng = random.Random(7)
+    for n in (1, 2, 5, 10, 20):
+        for _ in range(20):
+            km.simulate_double_buffer(random.Random(rng.getrandbits(32)), n)
+    for _ in range(50):
+        km.simulate_tile_handoff(random.Random(rng.getrandbits(32)))
+    caught = 0
+    for _ in range(50):
+        try:
+            km.simulate_tile_handoff(random.Random(rng.getrandbits(32)), barrier=False)
+        except AssertionError:
+            caught += 1
+    assert caught >= 30
 
 
 def test_two_slot_fused_temporal_attention_barrier_protocol_model():
-    """tattn_fused2_kernel: two convert / softmax warpgroups on alternate items, each TMEM slot's accumulator columns re-used in place
-    (Q fp16 over Q, S over the K / V accumulators, P over S), MMA order S(i) PV(i-1) QKV(i+1): no deadlock, no aliasing hazard under
-    randomised latencies — and the model does catch a wrong order (QKV(i+1) issued before PV(i-1))."""
-    import random
-    from tools import protocol_sim
-    rng = random.Random(11)
-    for items, num_kb, stages in ((1, 5, 4), (2, 5, 4), (3, 5, 4), (7, 10, 4), (4, 1, 2), (10, 8, 3)):
-        for _ in range(6):
-            protocol_sim.simulate_tfused2(random.Random(rng.getrandbits(32)), items, num_kb, stages)
-    caught = 0
-    for _ in range(10):  # negative control: the projection of item i + 1 issued while PV(i - 1) still owns the slot
-        try:
-            protocol_sim.simulate_tfused2(random.Random(rng.getrandbits(32)), 6, 5, 4, wrong_order=True)
-        except AssertionError:
-            caught += 1
-    assert caught == 10
+    """tattn_fused_kernel packs 128 / F pixels into the 128 query slots and lets each warpgroup visit only the key tiles its
+    sequences can reach (kt = wg when F <= 64, both 64-slot tiles when F = 128): for every F dividing 128 each query row keeps
+    exactly the F keys of its own pixel — and the model catches the wrong half (kt = 1 - wg)."""
+    from tools import kernel_models as km
+    for F in (1, 2, 4, 8, 16, 32, 64, 128):
+        km.check_fused_key_tiles(F)
+    for F in (1, 8, 16, 64):
+        with pytest.raises(AssertionError):
+            km.check_fused_key_tiles(F, wrong=True)
 
 
 def test_lean_gemm_epilogue_bookkeeping_model():
-    """tools/epilogue_schedule_model.py restates the counters of the lean GEMM epilogue (division-free tile iterator, chunk ownership of
-    the two groups with the alternating odd chunk, residual prefetch cursor, output staging ring + rotating store issuer) and checks
-    them against the plain definitions for the tile shapes of the step, ragged N, GEGLU pairs and both staging depths."""
-    from tools import epilogue_schedule_model as m
-    visits = 0
-    for BN, N, geglu in ((160, 960, False), (160, 320, False), (256, 2560, True), (128, 320, False), (64, 200, False), (256, 1280, False),
-                         (128, 1280, True), (160, 1000, False)):
-        n_tiles = (N + BN - 1) // BN
-        for first, stride, m_units in ((0, 148, 1536), (147, 148, 1536), (3, 7, 40), (5, 74, 193), (0, 1, 3)):
-            for k_ob in (2, 3):
-                visits += m.check(first, stride, m_units, n_tiles, N, BN, geglu, k_ob)
-    assert visits > 10000
+    """gemm_wgmma_kernel: (1) the cp.async stage ring with the stage count, wait_group depth and prefetch distance read from
+    csrc/gemm_wgmma.cu — every block lands before a wgmma reads it and no slot is refilled before both warpgroups retired the
+    wgmma that read it, under randomised latencies; a prefetch one block further or a laxer wait_group is caught; (2) the
+    register epilogue's index arithmetic: accumulator layout, GEGLU (h, gate) pairing against geglu_pack, up2 phase rows."""
+    import random
+    from tools import kernel_models as km
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import kernel_contracts
+    stages, wait_depth, dist = km.gemm_pipeline_constants()
+    rng = random.Random(11)
+    for nk in (1, 2, 3, 5, 9, 20, 45):
+        for _ in range(20):
+            km.simulate_gemm_ring(random.Random(rng.getrandbits(32)), nk, stages, wait_depth, dist)
+    for bad in (dict(stages=stages, wait_depth=wait_depth, dist=dist + 1), dict(stages=stages, wait_depth=wait_depth + 1, dist=dist)):
+        caught = 0
+        for _ in range(20):
+            try:
+                km.simulate_gemm_ring(random.Random(rng.getrandbits(32)), 20, **bad)
+            except AssertionError:
+                caught += 1
+        assert caught >= 15, bad
+    km.check_epilogue(kernel_contracts.geglu_pack)
 
 
 def test_fma_pipe_exp2_polynomial_emulation():
-    """ex2_poly of csrc/ptx.cuh (used by attention2q / attention_v10) emulated in float32 / int32: accuracy far below fp16 resolution, and no
+    """ex2_poly of csrc/ptx.cuh (used by csrc/attention_wgmma.cu) emulated in float32 / int32: accuracy far below fp16 resolution, and no
     exponent-field wrap-around for masked keys (-inf) — the clamp must stay at -125 (see the kernel comment)."""
     from tools import exp2_poly_fit
     rel, masked = exp2_poly_fit.check()
@@ -387,9 +387,9 @@ def test_fma_pipe_exp2_polynomial_emulation():
 
 @pytest.mark.parametrize("poly", [0, 1, 2])
 def test_attn2q_algorithm_emulation(poly):
-    """tools/attn2q_emulation.py: the per-row algorithm of csrc/attention2q_tcgen05.cu (128-key tiles, thresholded running
-    max with O / l rescale, fp16 P, FMA-pipe exp2 on 0 / 25 / 50 % of the elements, key-tail masks) against exact softmax
-    attention at the tolerance of the GPU parity tests."""
-    from tools import attn2q_emulation as em
+    """tools/attention_emulation.py: the per-row algorithm of csrc/attention_wgmma.cu (64-key tiles, running max raised on every
+    tile with O / l rescale, fp16 P, FMA-pipe exp2 on 0 / 25 (the kernel's split) / 50 % of the elements, key-tail masks) against
+    exact softmax attention at the tolerance of the GPU parity tests."""
+    from tools import attention_emulation as em
     for kw in (dict(T=64, L=300), dict(T=128, L=145), dict(T=64, L=512, mag=6.0), dict(T=64, L=640, rising=True)):
         assert em.check(poly=poly, **kw) < 0.5, (poly, kw)

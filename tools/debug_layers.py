@@ -1,4 +1,4 @@
-"""Layer-by-layer comparison of the B200 UNet against the oracle (development aid)."""
+"""Layer-by-layer comparison of this package's UNet against the oracle (development aid)."""
 import sys
 
 import torch

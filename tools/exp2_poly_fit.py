@@ -1,4 +1,4 @@
-"""Fit and check the FMA-pipe exp2 of csrc/attention2q_tcgen05.cu (ex2_poly): Cody-Waite split x = n + f with the
+"""Fit and check the FMA-pipe exp2 of csrc/ptx.cuh (ex2_poly, used by csrc/attention_wgmma.cu): Cody-Waite split x = n + f with the
 1.5 * 2^23 rounding trick, degree-3 minimax polynomial for 2^f on [-0.5, 0.5], exponent-field add for 2^n.
 Emulated in float32 / int32 numpy exactly as the device code computes it (fma -> mul+add: one extra rounding, which only
 loosens this check).  Run: python tools/exp2_poly_fit.py"""

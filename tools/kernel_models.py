@@ -1,0 +1,178 @@
+"""CPU models of the synchronisation and index bookkeeping of the sm_90a kernels (csrc/gemm_wgmma.cu, csrc/attention_wgmma.cu).
+
+A data race or a wrong index in these kernels shows up on the GPU only as occasionally wrong numbers, so the schedules are
+restated here as discrete-event models with randomised latencies and checked for their hazards, each with a negative control
+(the same model with one rule broken must be caught).  The pipeline constants are read from the kernel sources, so a change
+there that breaks a rule fails here.
+"""
+from __future__ import annotations
+
+import os
+import random
+import re
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+CSRC = os.path.join(ROOT, "anyv2v_b200", "csrc")
+
+
+def _src(name):
+    return open(os.path.join(CSRC, name)).read()
+
+
+def gemm_pipeline_constants():
+    """(stages, wait_group depth, prefetch distance) of the GEMM's cp.async ring, as written in gemm_wgmma.cu"""
+    s = _src("gemm_wgmma.cu")
+    stages = int(re.search(r"constexpr int kStages = (\d+);", s).group(1))
+    wait = eval(re.search(r"cp_async_wait<(kStages - \d+)>\(\);\n\s*fence_proxy_async_smem", s).group(1), {"kStages": stages})
+    dist = eval(re.search(r"const int pf = kb \+ (kStages - \d+);", s).group(1), {"kStages": stages})
+    return stages, wait, dist
+
+
+# ---------------------------------------------------------------------------------------------------------- GEMM ring
+def simulate_gemm_ring(rng: random.Random, nk: int, stages: int, wait_depth: int, dist: int, n_wg: int = 2):
+    """gemm_wgmma_kernel's K loop.  Per K block kb, every thread: cp.async.wait_group(wait_depth) -> fence -> __syncthreads ->
+    issue the loads of block kb + dist into slot (kb + dist) % stages, commit -> wgmma kb on slot kb % stages, commit ->
+    wgmma.wait_group(1) (wgmma kb - 1 retired).  Asserts: a block is landed before any wgmma reads it, and a slot is
+    overwritten only after every warpgroup retired the wgmma that read it."""
+    land = {}
+    groups = []  # one cp.async group per prologue stage / iteration, in commit order: the block it loads or None
+    retire = [dict() for _ in range(n_wg)]
+    t_wg = [0.0] * n_wg
+    for s in range(dist):
+        land[s] = rng.uniform(1, 50) if s < nk else 0.0
+        groups.append(s if s < nk else None)
+    for kb in range(nk):
+        for w in range(n_wg):  # wait_group(wait_depth): all but the newest wait_depth groups have landed
+            done = groups[:len(groups) - wait_depth] if wait_depth else groups
+            t_wg[w] = max([t_wg[w]] + [land[g] for g in done if g is not None])
+        T = max(t_wg)  # __syncthreads
+        j = kb + dist
+        if j < nk:
+            prev = j - stages  # the block that last occupied slot j % stages
+            if prev >= 0:
+                for w in range(n_wg):
+                    assert retire[w][prev] <= T, f"slot {j % stages} overwritten by block {j} while block {prev} is still read"
+            land[j] = T + rng.uniform(1, 50)
+            groups.append(j)
+        else:
+            groups.append(None)
+        assert land[kb] <= T, f"wgmma reads block {kb} before its cp.async landed"
+        for w in range(n_wg):
+            issue = T + rng.uniform(0, 3)
+            retire[w][kb] = issue + rng.uniform(1, 40)
+            t_wg[w] = max(issue, retire[w].get(kb - 1, 0.0))  # wgmma.wait_group(1)
+    return True
+
+
+# ---------------------------------------------------------------------------------------------------------- double buffer
+def simulate_double_buffer(rng: random.Random, n: int, trailing_barrier: bool = True, n_wg: int = 2):
+    """The K/V loop of attn_kernel and the projection loop of tattn_fused_kernel (project): load 0; per step kt: issue the
+    loads of kt + 1 into buffer (kt + 1) & 1, commit, wait_group(1) (wait_group(0) on the last step) -> fence ->
+    __syncthreads -> every warpgroup computes on buffer kt & 1 -> __syncthreads.  Asserts the same two hazards as the GEMM
+    ring; without the trailing barrier a fast warpgroup's prefetch overwrites the buffer a slow one still reads."""
+    land = {0: rng.uniform(1, 50)}
+    reads = {}  # step -> per-warpgroup end of compute
+    t_wg = [0.0] * n_wg
+    for kt in range(n):
+        for w in range(n_wg):
+            if kt + 1 < n:  # each thread issues its share of the next step's loads on arrival
+                prev = kt - 1
+                if prev >= 0:
+                    for w2 in range(n_wg):
+                        assert reads[prev][w2] <= t_wg[w], f"buffer {(kt + 1) & 1} overwritten while step {prev} reads it"
+                land[kt + 1] = max(land.get(kt + 1, 0.0), t_wg[w] + rng.uniform(1, 50))
+            t_wg[w] = max(t_wg[w], land[kt])  # wait_group(1): the group of step kt landed
+        T = max(t_wg)  # __syncthreads
+        assert land[kt] <= T
+        reads[kt] = [T + rng.uniform(1, 60) for _ in range(n_wg)]
+        t_wg = list(reads[kt])
+        if trailing_barrier:
+            t_wg = [max(t_wg)] * n_wg
+    return True
+
+
+def simulate_tile_handoff(rng: random.Random, barrier: bool = True, n_wg: int = 2):
+    """tattn_fused_kernel between projection and attention: each warpgroup stores ITS 64 rows of the Q, K and V tiles
+    (acc_to_tile), then fence + __syncthreads, then each warpgroup's attention reads key / value rows of BOTH halves (F = 128
+    sequences span them).  Asserts every row is written before it is read."""
+    written = [rng.uniform(1, 80) for _ in range(n_wg)]  # end of each warpgroup's tile stores
+    start = [w_end + rng.uniform(0, 5) for w_end in written]
+    if barrier:
+        start = [max(written)] * n_wg
+    for w in range(n_wg):
+        for owner in range(n_wg):
+            assert written[owner] <= start[w], f"warpgroup {w} reads rows of warpgroup {owner} before they are stored"
+    return True
+
+
+# ---------------------------------------------------------------------------------------------------------- fused key tiles
+def fused_key_tiles(F: int, wg: int, wrong: bool = False):
+    """key tiles (64 slots each) the warpgroup wg visits in tattn_fused_kernel, as in the kernel: kt = wg when F <= 64 (a
+    sequence never crosses the 64-slot halves), else both"""
+    if F <= 64:
+        return [1 - wg if wrong else wg]
+    return [0, 1]
+
+
+def check_fused_key_tiles(F: int, wrong: bool = False):
+    """every key of a query slot's own pixel (slot // F equal) lies in a visited tile, and the kept keys per row are exactly F"""
+    for wg in range(2):
+        tiles = fused_key_tiles(F, wg, wrong)
+        for r in range(64):
+            q = wg * 64 + r
+            kept = [64 * kt + c for kt in tiles for c in range(64) if q // F == (64 * kt + c) // F]
+            assert len(kept) == F and all(k // F == q // F for k in kept), (F, wg, r, len(kept))
+    return True
+
+
+# ---------------------------------------------------------------------------------------------------------- GEMM epilogue
+def acc_row(t, i):
+    """ptx.cuh acc_row for warpgroup thread t: accumulator element i of wgmma m64nN"""
+    return 16 * (t >> 5) + ((t & 31) >> 2) + 8 * ((i >> 1) & 1)
+
+
+def acc_col(t, i):
+    return 8 * (i >> 2) + 2 * (t & 3) + (i & 1)
+
+
+def check_epilogue(geglu_pack, N_geglu=(128, 256, 2560)):
+    """gemm_wgmma_kernel's epilogue index arithmetic: (1) the accumulator layout maps the 128 threads x 64 registers of a
+    warpgroup one-to-one onto its 64 x 128 block; (2) GEGLU: the (h, gate) columns the kernel pairs (jh, jg = jh + 4 inside
+    each 64-column group, output column n0 / 2 + 32 g + 8 jj + cq) are the pairs geglu_pack interleaved, every output column
+    written once; (3) the up2 phase store maps the low-resolution pixels one-to-one onto the phase's pixels of the output."""
+    import torch
+    seen = {(acc_row(t, i), acc_col(t, i)) for t in range(128) for i in range(64)}
+    assert len(seen) == 64 * 128 and all(0 <= r < 64 and 0 <= c < 128 for r, c in seen)
+    for N in N_geglu:
+        inner = N // 2
+        w = torch.arange(N, dtype=torch.float64)[:, None]  # row n of W holds the value n: the packed order is visible
+        wp, _ = geglu_pack(w, torch.zeros(N, dtype=torch.float64))
+        packed = wp[:, 0].long().tolist()
+        out_cols = {}
+        for n0 in range(0, N, 128):
+            for t in range(128):
+                cq = 2 * (t & 3)
+                for g in range(2):
+                    for jj in range(4):
+                        jh, jg = 8 * g + jj, 8 * g + jj + 4
+                        ch, cg = n0 + 8 * jh + cq, n0 + 8 * jg + cq
+                        if ch >= N:
+                            continue
+                        oc = n0 // 2 + 32 * g + 8 * jj + cq
+                        for e in range(2):
+                            h_src, g_src = packed[ch + e], packed[cg + e]
+                            assert h_src < inner and g_src == h_src + inner, (N, ch, cg)
+                            assert out_cols.setdefault(oc + e, h_src) == h_src
+                            assert oc + e == h_src, (N, oc + e, h_src)  # output column j = h_j * gelu(gate_j)
+        assert sorted(out_cols) == list(range(inner))
+    for NF, H, W in ((2, 3, 5), (1, 8, 8), (3, 4, 16)):
+        for ph in range(4):
+            py, px = ph >> 1, ph & 1
+            rows = set()
+            for m in range(NF * H * W):
+                j, t = m % W, m // W
+                i, n = t % H, t // H
+                rows.add((n * 2 * H + 2 * i + py) * (2 * W) + 2 * j + px)
+            want = {(n * 2 * H + y) * (2 * W) + x for n in range(NF) for y in range(py, 2 * H, 2) for x in range(px, 2 * W, 2)}
+            assert rows == want
+    return True
