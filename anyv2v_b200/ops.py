@@ -72,6 +72,53 @@ def _f16_cuda(t: torch.Tensor, name: str) -> None:
         raise L.Av2vError(f"{name}: expected a CUDA fp16 tensor, got {t.device}/{t.dtype} (no CPU fallback exists)")
 
 
+def _require(cond: bool, msg: str) -> None:
+    if not cond:
+        raise L.Av2vError(msg)
+
+
+def _row_layout(t: torch.Tensor, name: str, rows: int, cols: int, slots: int = 1, slot_stride: int = 0) -> int:
+    """Row stride `ld` of `t` when t addresses element (s, m, n) at s * slot_stride + m * ld + n for s < slots, m < rows,
+    n < cols: the layout the kernels store (and read residuals) in.  Leading dims that nest exactly are merged, so an
+    [NF, H, W, C] image with a row stride, or a [slots, M, N] stack with a gap between slots, qualifies."""
+    _f16_cuda(t, name)
+    _require(t.dim() >= 2 and t.shape[-1] == cols and t.stride(-1) == 1,
+             f"{name}: expected [..., {cols}] with unit column stride, got shape {tuple(t.shape)} strides {t.stride()}")
+    groups = []  # (size, stride) of the leading dims, innermost first
+    for size, st in zip(reversed(t.shape[:-1]), reversed(t.stride()[:-1])):
+        if size == 1:
+            continue
+        if groups and st == groups[-1][0] * groups[-1][1]:
+            groups[-1] = (groups[-1][0] * size, groups[-1][1])
+        else:
+            groups.append((size, st))
+    groups = groups[::-1]
+    if rows == 1:
+        ld = cols
+        ok = groups == ([(slots, slot_stride)] if slots > 1 else [])
+    else:
+        ld = groups[-1][1] if groups else 0
+        ok = groups == ([(slots, slot_stride), (rows, ld)] if slots > 1 else [(rows, ld)]) or (
+            slots > 1 and groups == [(slots * rows, ld)] and slot_stride == rows * ld)
+    _require(ok and ld >= cols, f"{name}: shape {tuple(t.shape)} strides {t.stride()} does not hold "
+                                f"{slots} x [{rows}, {cols}] rows (slot stride {slot_stride})")
+    return ld
+
+
+def _vector(t: Optional[torch.Tensor], name: str, n: int) -> None:
+    if t is not None:
+        _f16_cuda(t, name)
+        _require(t.is_contiguous() and t.numel() == n, f"{name}: expected {n} contiguous elements, got shape {tuple(t.shape)}")
+
+
+def _rowbias(t: Optional[torch.Tensor], M: int, N: int, rows_per_rowbias: int) -> None:
+    if t is not None:
+        _f16_cuda(t, "rowbias")
+        _require(rows_per_rowbias > 0, "rowbias needs rows_per_rowbias > 0")
+        want = (-(-M // rows_per_rowbias), N)
+        _require(t.is_contiguous() and tuple(t.shape) == want, f"rowbias: expected a contiguous {want}, got {tuple(t.shape)}")
+
+
 # ----------------------------------------------------------------------------------------------------------- K7
 def ddim_step(x, v_neg, v_edit, guidance: float, ca: float, cb: float, cc: float, cd: float, out=None,
               inverse: bool = False, coef_dev=None):
@@ -85,6 +132,8 @@ def ddim_step(x, v_neg, v_edit, guidance: float, ca: float, cb: float, cc: float
         assert v_edit.is_contiguous() and v_edit.numel() == x.numel()
     if out is None:
         out = torch.empty_like(x)
+    _f16_cuda(out, "ddim_step.out")
+    _require(out.is_contiguous() and out.numel() == x.numel(), f"ddim_step.out: expected {x.numel()} contiguous elements")
     if coef_dev is not None:
         assert coef_dev.is_cuda and coef_dev.dtype == torch.float32 and coef_dev.numel() >= 5
     a = L.DdimArgs(_p(x), _p(v_neg), _p(v_edit), _p(out), x.numel(), guidance, ca, cb, cc, cd, _p(coef_dev))
@@ -110,6 +159,10 @@ def groupnorm(x, gamma, beta, groups: int, eps: float, silu: bool, out=None, x2=
         C = C1 + x2.shape[2]
     if out is None:
         out = torch.empty((n, rows, C), dtype=x.dtype, device=x.device)
+    _f16_cuda(out, "groupnorm.out")
+    _require(out.is_contiguous() and tuple(out.shape) == (n, rows, C), f"groupnorm.out: expected a contiguous {(n, rows, C)}")
+    _vector(gamma, "groupnorm.gamma", C)
+    _vector(beta, "groupnorm.beta", C)
     need = L.lib().av2v_groupnorm_workspace_floats(n, C)
     key = x.device.index
     ws = _gn_ws.get(key)
@@ -146,18 +199,21 @@ def linear(a, w, bias=None, residual=None, out=None, rowbias=None, rows_per_rowb
         _f16_cuda(a2, "linear.a2")
         assert a2.dim() == 2 and a2.stride(1) == 1 and a2.shape[0] == M and K % 64 == 0
         K = K + a2.shape[1]
+    _f16_cuda(w, "linear.w")
     N = w.shape[0]
     assert w.shape[1] == K
     if out is None:
         out = torch.empty((M, N // 2 if geglu else N), dtype=torch.float16, device=a.device)
-    assert out.stride(1) == 1
+    ldo = _row_layout(out, "linear.out", M, N // 2 if geglu else N)
     if residual is not None:
-        assert residual.stride(1) == 1 and residual.stride(0) == out.stride(0)
+        _require(_row_layout(residual, "linear.residual", M, N) == ldo, "linear.residual: row stride differs from out's")
+    _vector(bias, "linear.bias", N)
+    _rowbias(rowbias, M, N, rows_per_rowbias)
     g = L.GemmArgs()
     g.mode = L.A_LINEAR
     g.a, g.w, g.M, g.N, g.K, g.lda = _p(a), _p(w), M, N, K, a.stride(0)
     g.bias, g.rowbias, g.rows_per_rowbias = _p(bias), _p(rowbias), rows_per_rowbias
-    g.residual, g.out, g.ldo, g.n_slots, g.slot_stride = _p(residual), _p(out), out.stride(0), 1, 0
+    g.residual, g.out, g.ldo, g.n_slots, g.slot_stride = _p(residual), _p(out), ldo, 1, 0
     g.geglu = 1 if geglu else 0
     if a2 is not None:
         g.a2, g.k_split, g.lda2 = _p(a2), a.shape[1], a2.stride(0)
@@ -184,6 +240,10 @@ def layernorm(x, gamma, beta, eps: float = 1e-5, out=None):
     rows = x.numel() // C
     if out is None:
         out = torch.empty_like(x)
+    _f16_cuda(out, "layernorm.out")
+    _require(out.is_contiguous() and out.shape == x.shape, f"layernorm.out: expected a contiguous {tuple(x.shape)}")
+    _vector(gamma, "layernorm.gamma", C)
+    _vector(beta, "layernorm.beta", C)
     a = L.LayerNormArgs(_p(x), _p(out), _p(gamma), _p(beta), rows, C, eps)
     with _timed(f"layernorm rows={rows} C={C}"):
         L.check(L.lib().av2v_layernorm_f16(ctypes.byref(a), _stream()), "av2v_layernorm_f16")
@@ -195,8 +255,10 @@ def conv3x3(x, w_packed, bias=None, rowbias=None, rows_per_rowbias: int = 0, res
             n_slots: int = 1, slot_stride: int = 0, stride: int = 1):
     """3x3 / pad 1 convolution as an implicit GEMM. x: [NF,H,W,C] contiguous (channels-last),
     w_packed: [Cout, 9*Cin] (= conv.weight.permute(0,2,3,1).reshape). out: [n_slots][NF*(H/stride)*(W/stride), Cout].
-    stride 2 = Downsample2D (the taps are sampled with TMA element strides).  C < Cin (conv_in: 8 channels): the weights are
-    zero-padded per tap to Cin = 64 and the missing channels of every K block read as zeros (TMA out-of-bounds fill)."""
+    out (and residual, in the same layout) may have a row stride; with n_slots > 1, slot s starts slot_stride elements after
+    slot s - 1.  stride 2 = Downsample2D (each A row gathers the taps at twice the output coordinates).  C < Cin (conv_in: 8
+    channels): the weights are zero-padded per tap to Cin = 64 and the missing channels of every K block are zero-filled by
+    the cp.async channel predicate, as are out-of-image taps."""
     _f16_cuda(x, "conv3x3.x")
     assert x.dim() == 4 and x.is_contiguous()
     NF, H, W, C = x.shape
@@ -208,13 +270,19 @@ def conv3x3(x, w_packed, bias=None, rowbias=None, rows_per_rowbias: int = 0, res
     if out is None:
         assert n_slots == 1
         out = torch.empty((NF, H // stride, W // stride, Cout), dtype=torch.float16, device=x.device)
+    ldo = _row_layout(out, "conv3x3.out", M, Cout, n_slots, slot_stride)
+    if residual is not None:
+        _require(_row_layout(residual, "conv3x3.residual", M, Cout, n_slots, slot_stride) == ldo,
+                 "conv3x3.residual: row stride differs from out's")
+    _vector(bias, "conv3x3.bias", Cout)
+    _rowbias(rowbias, M, Cout, rows_per_rowbias)
     g = L.GemmArgs()
     g.mode = L.A_CONV3X3
     g.a, g.w, g.M, g.N, g.K = _p(x), _p(w_packed), M, Cout, 9 * Cin
     g.NF, g.H, g.W, g.Cin = NF, H, W, Cin
     g.stride, g.a_channels = stride, (C if C != Cin else 0)
     g.bias, g.rowbias, g.rows_per_rowbias = _p(bias), _p(rowbias), rows_per_rowbias
-    g.residual, g.out, g.ldo, g.n_slots, g.slot_stride = _p(residual), _p(out), Cout, n_slots, slot_stride
+    g.residual, g.out, g.ldo, g.n_slots, g.slot_stride = _p(residual), _p(out), ldo, n_slots, slot_stride
     _gemm(g)
     return out
 
@@ -232,12 +300,15 @@ def upsample2x_conv3x3(x, w_phases, bias=None, out=None):
     assert w_phases.shape[2] == 4 * Cin
     if out is None:
         out = torch.empty((NF, 2 * H, 2 * W, Cout), dtype=torch.float16, device=x.device)
+    ldo = _row_layout(out, "upsample2x_conv3x3.out", NF * 4 * H * W, Cout)
+    _require(out.dim() == 4 and tuple(out.shape[:3]) == (NF, 2 * H, 2 * W), f"upsample2x_conv3x3.out: expected {(NF, 2 * H, 2 * W, Cout)}")
+    _vector(bias, "upsample2x_conv3x3.bias", Cout)
     for ph in range(4):
         g = L.GemmArgs()
         g.mode = L.A_CONV3X3
         g.a, g.w, g.M, g.N, g.K = _p(x), _p(w_phases[ph]), NF * H * W, Cout, 4 * Cin
         g.NF, g.H, g.W, g.Cin = NF, H, W, Cin
-        g.bias, g.out, g.ldo, g.n_slots, g.slot_stride = _p(bias), _p(out), Cout, 1, 0
+        g.bias, g.out, g.ldo, g.n_slots, g.slot_stride = _p(bias), _p(out), ldo, 1, 0
         g.up2_phase = ph + 1
         _gemm(g)
     return out
@@ -273,16 +344,27 @@ def tconv3(x, w_packed, F: int, HW: int, bias=None, residual=None, out=None):
     assert w_packed.shape[1] == 3 * Cin and w_packed.is_contiguous()
     if out is None:
         out = torch.empty((B, R, Cout), dtype=torch.float16, device=x.device)
+    ldo = _row_layout(out, "tconv3.out", B * R, Cout)
+    if residual is not None:
+        _require(_row_layout(residual, "tconv3.residual", B * R, Cout) == ldo, "tconv3.residual: row stride differs from out's")
+    _vector(bias, "tconv3.bias", Cout)
     g = L.GemmArgs()
     g.mode = L.A_TCONV3
     g.a, g.w, g.M, g.N, g.K = _p(x), _p(w_packed), B * R, Cout, 3 * Cin
     g.B, g.rows_per_clip, g.HW, g.Cin = B, R, HW, Cin
-    g.bias, g.residual, g.out, g.ldo, g.n_slots, g.slot_stride = _p(bias), _p(residual), _p(out), Cout, 1, 0
+    g.bias, g.residual, g.out, g.ldo, g.n_slots, g.slot_stride = _p(bias), _p(residual), _p(out), ldo, 1, 0
     _gemm(g)
     return out
 
 
 # ----------------------------------------------------------------------------------------------------------- attention
+def _reach(t: torch.Tensor, name: str, rows: int, cols: int, offset: int = 0) -> None:
+    """a 2-D token matrix must hold columns [0, cols) and reach element offset + (rows - 1) * ld + cols - 1 of its storage"""
+    ld = t.stride(0)
+    _require(t.shape[1] >= cols and (t.shape[0] - 1) * ld + t.shape[1] >= offset + (rows - 1) * ld + cols,
+             f"{name}: shape {tuple(t.shape)} (row stride {ld}) does not cover {rows} rows x {cols} columns at offset {offset}")
+
+
 def attention(q, k, v, heads: int, seq: int, batch: int, out, scale: float = 0.125, n_v: int = 1,
               v_branch_stride: int = 0, o_branch_stride: int = 0, frames_mode: bool = False, HW: int = 0,
               seq_kv: int = 0, kv_batch_div: int = 0):
@@ -291,6 +373,12 @@ def attention(q, k, v, heads: int, seq: int, batch: int, out, scale: float = 0.1
     for name, t in (("q", q), ("k", k), ("v", v), ("o", out)):
         _f16_cuda(t, "attention." + name)
         assert t.dim() == 2 and t.stride(1) == 1
+    C, extra = heads * 64, n_v - 1
+    kv_rows = batch * seq if frames_mode else batch // max(kv_batch_div, 1) * (seq_kv if seq_kv > 0 else seq)
+    _reach(q, "attention.q", batch * seq, C)
+    _reach(k, "attention.k", kv_rows, C)
+    _reach(v, "attention.v", kv_rows, C, extra * v_branch_stride)
+    _reach(out, "attention.o", batch * seq, C, extra * o_branch_stride)
     a = L.AttnArgs()
     a.seq_mode = L.SEQ_FRAMES if frames_mode else L.SEQ_ROWS
     a.q, a.k, a.v, a.o = _p(q), _p(k), _p(v), _p(out)
@@ -314,6 +402,7 @@ def temporal_attention_fused(x, wqkv, heads: int, F: int, HW: int, clips: int, o
         assert t.dim() == 2 and t.stride(1) == 1
     assert wqkv.is_contiguous() and wqkv.shape[0] == 3 * heads * 64 and wqkv.shape[1] == x.shape[1]
     assert x.shape[0] == clips * F * HW == out.shape[0]
+    _require(out.shape[1] >= heads * 64, f"temporal_attention_fused.o: {out.shape[1]} columns, the heads need {heads * 64}")
     a = L.TAttnFusedArgs(_p(x), _p(wqkv), _p(out), x.stride(0), out.stride(0), clips, F, HW, heads, x.shape[1], scale, n_v)
     with _timed(f"temporal attention fused nv={n_v} clips={clips} F={F} HW={HW} heads={heads} Cx={x.shape[1]}"):
         L.check(L.lib().av2v_tattn_fused_f16(ctypes.byref(a), _stream()), "av2v_tattn_fused_f16")

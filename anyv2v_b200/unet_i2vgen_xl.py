@@ -72,7 +72,7 @@ class Conv3x3(nn.Conv2d):
 
     Widths the tensor-core tiles do not cover are padded in the PACKED weight only (the parameter keeps its diffusers shape):
     Cin not a multiple of 64 (conv_in: 8 input channels) -> every tap's K block is zero-padded to 64 and the activation's missing
-    channels read as zeros through TMA out-of-bounds fill; Cout not a multiple of 8 (conv_out: 4) -> zero rows up to 8 and the
+    channels are zero-filled by the GEMM's cp.async channel predicate; Cout not a multiple of 8 (conv_out: 4) -> zero rows up to 8 and the
     caller slices the result."""
 
     def __init__(self, cin, cout, stride: int = 1):

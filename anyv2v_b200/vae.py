@@ -33,7 +33,7 @@ SD_VAE_CONFIG = dict(in_channels=3, out_channels=3, latent_channels=4, block_out
 
 class LibConv2d(nn.Conv2d):
     """The VAE's stem / head convolutions (3 -> 128, 128 -> 3 / 8, 4 -> 512 channels) stay on cuDNN: they run once per clip,
-    outside the denoising loops, and their channel counts (3) are below the 16-byte granularity of the TMA taps."""
+    outside the denoising loops, and their channel counts (3) are below the 16-byte granularity of the cp.async taps."""
 
     def forward_nhwc(self, x):
         return nr.conv2d_nhwc(x, self.weight, self.bias, stride=self.stride[0], padding=self.padding[0])

@@ -7,8 +7,9 @@ row-strided views), exact (float64) arithmetic on the fp16 inputs, one rounding 
 de-duplication / pruning switches can be checked for bit-identical results), and the
 ``emulated_ops`` fixture (tests/conftest.py) swaps it in for the duration of ONE test.  That lets the host logic that sits
 on top of the kernels (the channels-last UNet wiring, the PnP de-duplication, hooks, loops, latent store) run on CPU and
-be compared with the oracle.  The kernels themselves are checked against the same fp32 formulas on the GPU
-(tests/test_gpu_kernels.py); nothing outside tests/ imports this file.
+be compared with the oracle.  tests/test_gpu_contracts.py runs every kernel against these functions on the GPU (guarded
+buffers, same views and strides), so the contract the CPU tests rely on is the one the kernels implement;
+tests/test_gpu_kernels.py checks them against inline fp32 formulas as well.  Nothing outside tests/ imports this file.
 """
 from __future__ import annotations
 
@@ -151,12 +152,11 @@ def conv3x3(x, w_packed, bias=None, rowbias=None, rows_per_rowbias=0, residual=N
         if residual is not None:
             y = y + residual.double().reshape(M, Cout)
         return y.to(torch.float16).contiguous().view(NF, H, W, Cout)
-    flat = out.view(-1)
-    rflat = None if residual is None else residual.reshape(-1)
+    # slot s, row m lives at s * slot_stride + m * ld (ld = the row stride of out; the residual has out's layout)
+    rows = lambda t, s: t.as_strided((M, Cout), (t.stride(-2), 1), t.storage_offset() + s * slot_stride)
     for s in range(n_slots):  # one accumulator tile, n_slots stores (+ each slot's own residual): fused PnP injection
-        lo = s * slot_stride
-        ys = y if rflat is None else y + rflat[lo:lo + M * Cout].double().view(M, Cout)
-        flat[lo:lo + M * Cout] = ys.to(torch.float16).reshape(-1)
+        ys = y if residual is None else y + rows(residual, s).double()
+        rows(out, s).copy_(ys.to(torch.float16))
     return out
 
 

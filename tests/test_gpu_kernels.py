@@ -366,8 +366,8 @@ def test_groupnorm_sample_larger_than_l2(ops):
 
 @pytest.mark.parametrize("geo", [(48, 64, 64, 320, 320), (6, 32, 32, 640, 640), (4, 16, 16, 1280, 1280), (3, 8, 8, 128, 64), (5, 4, 4, 64, 128), (2, 2, 2, 64, 64)])
 def test_conv3x3_stride2(ops, geo):
-    """Downsample2D (Conv 3x3, stride 2, pad 1; diffusers downsampling.py, twin at seine/models/resnet.py:79-110): the taps are
-    sampled with TMA element strides, one output tile = box_h x W/2 output pixels"""
+    """Downsample2D (Conv 3x3, stride 2, pad 1; diffusers downsampling.py, twin at seine/models/resnet.py:79-110): every A row
+    gathers the taps of one output pixel at twice its coordinates with cp.async; out-of-image taps are zero-filled"""
     NF, H, W, Cin, Cout = geo
     torch.manual_seed(11)
     x = torch.randn(NF, H, W, Cin, device=dev).half()
@@ -381,7 +381,7 @@ def test_conv3x3_stride2(ops, geo):
 
 @pytest.mark.parametrize("geo", [(48, 64, 64, 8, 320), (4, 16, 16, 8, 64), (3, 32, 32, 24, 128), (16, 64, 64, 320, 4), (2, 16, 16, 64, 4)])
 def test_conv3x3_padded_channels(ops, geo):
-    """conv_in (8 -> 320: K blocks zero-padded to 64 channels, missing channels read as zeros by TMA) and conv_out (320 -> 4:
+    """conv_in (8 -> 320: K blocks zero-padded to 64 channels, the cp.async channel predicate zero-fills the missing ones) and conv_out (320 -> 4:
     weight rows zero-padded to 8, result sliced) through the product module"""
     from anyv2v_b200.unet_i2vgen_xl import Conv3x3
     NF, H, W, Cin, Cout = geo
