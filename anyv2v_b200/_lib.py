@@ -56,6 +56,11 @@ class TAttnFusedArgs(Structure):
                 ("F", c_int32), ("HW", c_int32), ("heads", c_int32), ("Cx", c_int32), ("scale", c_float), ("n_v", c_int32)]
 
 
+class FreeUArgs(Structure):
+    _fields_ = [("hidden", c_void_p), ("skip", c_void_p), ("out", c_void_p), ("NF", c_int32), ("H", c_int32), ("W", c_int32),
+                ("Ch", c_int32), ("Cs", c_int32), ("b", c_float), ("s", c_float)]
+
+
 #: every symbol include/anyv2v_b200.h declares -> (restype, argtypes)
 EXPORTS = {
     "av2v_abi_version": (c_int, []),
@@ -69,6 +74,7 @@ EXPORTS = {
     "av2v_layernorm_f16": (c_int, [POINTER(LayerNormArgs), c_void_p]),
     "av2v_attn_pnp_f16": (c_int, [POINTER(AttnArgs), c_void_p]),
     "av2v_tattn_fused_f16": (c_int, [POINTER(TAttnFusedArgs), c_void_p]),
+    "av2v_freeu_f16": (c_int, [POINTER(FreeUArgs), c_void_p]),
 }
 
 _lib = None

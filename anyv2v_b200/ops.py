@@ -357,6 +357,32 @@ def tconv3(x, w_packed, F: int, HW: int, bias=None, residual=None, out=None):
     return out
 
 
+# ----------------------------------------------------------------------------------------------------------- FreeU
+def freeu(hidden, skip, b: float, s: float, out=None):
+    """FreeU at one skip connection of up_blocks[0] / [1] (diffusers `apply_freeu`, csrc/freeu.cu): scales hidden[..., :Ch/2]
+    by b IN PLACE and returns fourier_filter(skip, threshold=1, scale=s).  hidden: [NF,H,W,Ch]; skip, out: [NF,H,W,Cs];
+    all contiguous (channels-last frames)."""
+    global _launches
+    _f16_cuda(hidden, "freeu.hidden")
+    _f16_cuda(skip, "freeu.skip")
+    _require(skip.dim() == 4 and skip.is_contiguous(), f"freeu.skip: expected a contiguous [NF, H, W, C], got shape "
+                                                        f"{tuple(skip.shape)} strides {skip.stride()}")
+    NF, H, W, Cs = skip.shape
+    _require(hidden.dim() == 4 and hidden.is_contiguous() and tuple(hidden.shape[:3]) == (NF, H, W),
+             f"freeu.hidden: expected a contiguous [{NF}, {H}, {W}, C], got shape {tuple(hidden.shape)} strides {hidden.stride()}")
+    if out is None:
+        out = torch.empty_like(skip)
+    _f16_cuda(out, "freeu.out")
+    _require(out.is_contiguous() and out.shape == skip.shape, f"freeu.out: expected a contiguous {tuple(skip.shape)}, got shape "
+                                                               f"{tuple(out.shape)} strides {out.stride()}")
+    _require(hidden.device == skip.device == out.device, "freeu: hidden, skip and out must be on the same device")
+    a = L.FreeUArgs(_p(hidden), _p(skip), _p(out), NF, H, W, hidden.shape[3], Cs, b, s)
+    with _timed(f"freeu NF={NF} H={H} W={W} Ch={hidden.shape[3]} Cs={Cs}"):
+        L.check(L.lib().av2v_freeu_f16(ctypes.byref(a), _stream()), "av2v_freeu_f16")
+    _launches += 1
+    return out
+
+
 # ----------------------------------------------------------------------------------------------------------- attention
 def _reach(t: torch.Tensor, name: str, rows: int, cols: int, offset: int = 0) -> None:
     """a 2-D token matrix must hold columns [0, cols) and reach element offset + (rows - 1) * ld + cols - 1 of its storage"""

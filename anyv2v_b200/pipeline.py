@@ -45,7 +45,7 @@ class _GraphedIteration:
     """One loop iteration captured as a CUDA graph (streams + graphs instead of a tracing compiler).
 
     The iteration body reads only static device buffers (latents, source latent, timestep, scheduler coefficients) so
-    the same graph is replayed for every timestep with the same hook-flag combination.  The first use runs eagerly
+    the same graph is replayed for every timestep with the same hook flags and FreeU setting.  The first use runs eagerly
     (allocates workspaces / packed weights, builds nothing under capture), the second captures, later ones replay."""
 
     def __init__(self, body, on_cuda: bool = True, pool=None):
@@ -171,6 +171,18 @@ class I2VGenXLPipeline:
             width, height = image.size
         return height, width
 
+    def enable_freeu(self, s1: float, s2: float, b1: float, b2: float):
+        """FreeU (arXiv:2309.11497), pipeline_i2vgen_xl.py:623-650: forwarded to ``unet.enable_freeu``.  s1 / s2 scale the low
+        frequencies of the skip features of up blocks 0 / 1, b1 / b2 the first half of their backbone channels.  Applies to
+        ``invert`` and ``sample_with_pnp``, also when switched between steps (e.g. from ``callback``)."""
+        if getattr(self, "unet", None) is None:
+            raise ValueError("The pipeline must have `unet` for using FreeU.")
+        self.unet.enable_freeu(s1=s1, s2=s2, b1=b1, b2=b2)
+
+    def disable_freeu(self):
+        """Disables FreeU if enabled (pipeline_i2vgen_xl.py:646-648)."""
+        self.unet.disable_freeu()
+
     def register_modules(self, **kwargs):
         for k, v in kwargs.items():
             setattr(self, k, v)
@@ -276,7 +288,9 @@ class I2VGenXLPipeline:
                 v = self.unet(st.latents, st.g_t, cond=st.cond)[0]
                 st.scheduler.step(v, None, st.latents, out=st.latents, coef_dev=st.g_coef)  # in place: x_t -> x_{t+1}
 
-        st.iteration = _GraphedIteration(body, on_cuda=st.latents.is_cuda)
+        st.body = body
+        st.iterations = {}  # FreeU setting -> _GraphedIteration
+        st.graph_pool = torch.cuda.graph_pool_handle() if st.latents.is_cuda else None
         return st
 
     def invert_step(self, st, i: int):
@@ -284,10 +298,14 @@ class I2VGenXLPipeline:
         t = st.timesteps[i]
         st.g_t.copy_(st.t_table[i:i + 1])
         st.g_coef.copy_(st.coef_table[i])
+        key = self.unet.freeu_state()
+        it = st.iterations.get(key)
+        if it is None:
+            it = st.iterations[key] = _GraphedIteration(st.body, on_cuda=st.latents.is_cuda, pool=st.graph_pool)
         if self.use_cuda_graphs:
-            st.iteration.run()
+            it.run()
         else:
-            st.iteration.body()
+            it.body()
         st.store.put(t, st.latents)
         return st.latents
 
@@ -385,7 +403,7 @@ class I2VGenXLPipeline:
         st.g_t = torch.zeros(1, device=dev, dtype=torch.int64)
         st.g_coef = torch.zeros(5, device=dev, dtype=torch.float32)
         st.g_src = torch.zeros_like(st.latents)
-        st.iterations = {}  # hook-flag combination -> _GraphedIteration
+        st.iterations = {}  # (dead source, hook flags, FreeU setting) -> _GraphedIteration
         st.graph_pool = torch.cuda.graph_pool_handle() if st.latents.is_cuda else None  # one activation pool for all of them
         # uncond and cond are the same latents + image latents -> they share the UNet prefix up to the first cross-attention
         # (I2VGenXLUNet.forward, shared_edit_prefix); the source branch is dropped after the last injection site that fires in
@@ -423,7 +441,8 @@ class I2VGenXLPipeline:
         t = st.timesteps[i]
         register_time(self, t)
         dead_source = st.skip and not st.fires[i]
-        key = (dead_source,) + self._hook_flags(t)
+        flags = self._hook_flags(t)
+        key = (dead_source, flags, self.unet.freeu_state())
         it = st.iterations.get(key)
         if it is None:
             if dead_source:
@@ -432,7 +451,7 @@ class I2VGenXLPipeline:
                                   shared_edit_prefix=st.shared_prefix)[0]
                     st.scheduler.step(v[0:1], None, st.latents, model_output_cond=v[1:2], out=st.latents, coef_dev=st.g_coef)
             else:
-                site = self._prune_site(key[1:]) if st.prune_source else None
+                site = self._prune_site(flags) if st.prune_source else None
                 lo = 0 if site is not None else 1  # the pruned forward returns [uncond, cond] only
 
                 def body():

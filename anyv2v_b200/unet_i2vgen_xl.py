@@ -608,9 +608,11 @@ class DownBlock3D(_Block3D):
 
 
 class UpBlock3D(_Block3D):
-    def __init__(self, in_ch, out_ch, prev_ch, temb_ch, layers, hd, cross_dim, groups, attn, add_upsample):
+    def __init__(self, in_ch, out_ch, prev_ch, temb_ch, layers, hd, cross_dim, groups, attn, add_upsample, resolution_idx=None):
         super().__init__()
         self.has_cross_attention = attn
+        self.resolution_idx = resolution_idx
+        self.s1 = self.s2 = self.b1 = self.b2 = None  # FreeU factors (I2VGenXLUNet.enable_freeu)
         self.resnets = nn.ModuleList(
             ResnetBlock2D((prev_ch if i == 0 else out_ch) + (in_ch if i == layers - 1 else out_ch), out_ch, temb_ch, groups)
             for i in range(layers))
@@ -620,11 +622,21 @@ class UpBlock3D(_Block3D):
             self.temp_attentions = nn.ModuleList(TransformerTemporalModel(out_ch // hd, hd, out_ch, groups) for _ in range(layers))
         self.upsamplers = nn.ModuleList([Upsample2D(out_ch)]) if add_upsample else None
 
+    def freeu_factors(self):
+        """(b, s) of diffusers' `apply_freeu` at this block's skip connections, or None.  As in diffusers, FreeU is on when
+        s1, s2, b1 and b2 are all truthy (so a 0.0 turns it off), and only up blocks 0 and 1 change anything."""
+        if not (self.s1 and self.s2 and self.b1 and self.b2) or self.resolution_idx not in (0, 1):
+            return None
+        return (self.b1, self.s1) if self.resolution_idx == 0 else (self.b2, self.s2)
+
     def forward_nhwc(self, x, skips, temb, ctx, nframes, prune=None, block_index=None):
+        freeu = self.freeu_factors()
         for i in range(len(self.resnets)):
             skip = skips.pop()
             if skip.shape[0] != x.shape[0]:       # the source branch was pruned: keep the edit branches' frames
                 skip = skip[skip.shape[0] - x.shape[0]:]
+            if freeu is not None:                 # before the concat, so a patched (conv-injected) resnet sees it too
+                skip = ops.freeu(x, skip, *freeu)  # x[..., :C/2] *= b in place; Fourier-filtered copy of the skip
             x, temb, ctx = self._layer(i, x, temb, ctx, nframes, prune, block_index, skip=skip)
         if self.upsamplers is not None:
             x = self.upsamplers[0].forward_nhwc(x)
@@ -721,7 +733,7 @@ class I2VGenXLUNet(nn.Module):
         for i in range(n):
             prev, out_ch = out_ch, rev[i]
             self.up_blocks.append(UpBlock3D(rev[min(i + 1, n - 1)], out_ch, prev, temb, layers_per_block + 1, head_dim,
-                                            cross_attention_dim, g, attn=i > 0, add_upsample=i < n - 1))
+                                            cross_attention_dim, g, attn=i > 0, add_upsample=i < n - 1, resolution_idx=i))
         self.conv_norm_out = GroupNorm(g, c0, eps=1e-5)
         self.conv_act = nn.SiLU()
         self.conv_out = Conv3x3(c0, out_channels)
@@ -729,6 +741,22 @@ class I2VGenXLUNet(nn.Module):
     @property
     def dtype(self):
         return self.conv_in.weight.dtype
+
+    def enable_freeu(self, s1, s2, b1, b2):
+        """FreeU (arXiv:2309.11497), as diffusers' I2VGenXLUNet.enable_freeu: s1, s2, b1, b2 are set on every up block; at
+        each skip connection of up_blocks[0] (b1, s1) and up_blocks[1] (b2, s2) the first half of the backbone channels is
+        scaled by b and the skip's lowest frequencies by s."""
+        for blk in self.up_blocks:
+            blk.s1, blk.s2, blk.b1, blk.b2 = s1, s2, b1, b2
+
+    def disable_freeu(self):
+        for blk in self.up_blocks:
+            blk.s1 = blk.s2 = blk.b1 = blk.b2 = None
+
+    def freeu_state(self):
+        """the FreeU factors each up block applies (None where it applies none): a forward captured in a CUDA graph bakes
+        them in, so they are part of what selects a graph"""
+        return tuple(blk.freeu_factors() for blk in self.up_blocks)
 
     # -- conditioning that does not depend on the timestep or the latents: computed once per clip, not per step
     @torch.no_grad()

@@ -203,6 +203,23 @@ typedef struct {
 } av2v_tattn_fused_args;
 int av2v_tattn_fused_f16(const av2v_tattn_fused_args* a, av2v_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * FreeU at one skip connection of up_blocks[0] / up_blocks[1] (diffusers 0.26.3 `apply_freeu`, enabled through
+ * pipeline_i2vgen_xl.py:623-650 `enable_freeu`), applied before the skip concat:
+ *   hidden[..., :Ch/2] = fp16(fp32(hidden) * b)                       in place (torch's fp16 `x * b`)
+ *   out = fourier_filter(skip, threshold = 1, scale = s)               per (frame, channel) plane: the frequencies {0, -1}
+ *         of each axis (only {0} on a size-1 axis) scaled by s; closed form, seven fp32 sums per plane, no FFT, one
+ *         rounding to fp16.  Any H, W >= 1; Ch, Cs multiples of 8; all tensors contiguous and 16-byte aligned.
+ */
+typedef struct {
+  void* hidden;      /* [NF][H][W][Ch] */
+  const void* skip;  /* [NF][H][W][Cs] */
+  void* out;         /* [NF][H][W][Cs]: the filtered skip */
+  int32_t NF, H, W, Ch, Cs;
+  float b, s;
+} av2v_freeu_args;
+int av2v_freeu_f16(const av2v_freeu_args* a, av2v_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
