@@ -1,4 +1,4 @@
-// HBM-bound row kernels of the hot path: fused CFG + DDIM step (K7) and LayerNorm.  GroupNorm(+SiLU) (K6) is groupnorm.cu.
+// HBM-bound row kernels of the hot path: fused CFG + DDIM step (K7, eta = 0 and eta > 0) and LayerNorm.  GroupNorm(+SiLU) (K6) is groupnorm.cu.
 #include "host_util.cuh"
 #include "ptx.cuh"
 
@@ -25,16 +25,21 @@ __device__ __forceinline__ float ddim_one(float x, float vn, float ve, bool cfg,
   return r16(__fadd_rn(r16(__fmul_rn(cc, x0)), dir));
 }
 
+// kNoise: stochastic DDIM (eta > 0).  diffusers' step adds std_dev_t * variance_noise to the eta = 0 update as two more
+// PyTorch ops (fp32 0-dim scalar times fp16 tensor, then fp16 + fp16), so the kernel rounds twice more:
+// out = r16(ddim_one(...) + r16(cs * z)), with cd = sqrt(1 - a_prev - cs^2) passed in by the host.
+template <bool kNoise>
 __global__ void __launch_bounds__(256)
 ddim_step_kernel(const __half* __restrict__ x, const __half* __restrict__ vn, const __half* __restrict__ ve,
-                 __half* __restrict__ out, long long n, float g, float ca, float cb, float cc, float cd,
-                 const float* __restrict__ coef_dev) {
+                 const __half* __restrict__ z, __half* __restrict__ out, long long n, float g, float ca, float cb,
+                 float cc, float cd, float cs, const float* __restrict__ coef_dev) {
   if (coef_dev != nullptr) {
     ca = coef_dev[0];
     cb = coef_dev[1];
     cc = coef_dev[2];
     cd = coef_dev[3];
     g = coef_dev[4];
+    if (kNoise) cs = coef_dev[5];
   }
   const bool cfg = ve != nullptr;
   const long long nvec = n >> 3;
@@ -44,22 +49,38 @@ ddim_step_kernel(const __half* __restrict__ x, const __half* __restrict__ vn, co
     const uint4 nv = reinterpret_cast<const uint4*>(vn)[i];
     uint4 ev = nv;
     if (cfg) ev = reinterpret_cast<const uint4*>(ve)[i];
+    uint4 zv = nv;
+    if (kNoise) zv = reinterpret_cast<const uint4*>(z)[i];
     const __half* xh = reinterpret_cast<const __half*>(&xv);
     const __half* nh = reinterpret_cast<const __half*>(&nv);
     const __half* eh = reinterpret_cast<const __half*>(&ev);
+    const __half* zh = reinterpret_cast<const __half*>(&zv);
     uint4 ov;
     __half* oh = reinterpret_cast<__half*>(&ov);
 #pragma unroll
-    for (int e = 0; e < 8; ++e)
-      oh[e] = __float2half_rn(ddim_one(__half2float(xh[e]), __half2float(nh[e]), __half2float(eh[e]), cfg, g, ca,
-                                       cb, cc, cd));
+    for (int e = 0; e < 8; ++e) {
+      float y = ddim_one(__half2float(xh[e]), __half2float(nh[e]), __half2float(eh[e]), cfg, g, ca, cb, cc, cd);
+      if (kNoise) y = r16(__fadd_rn(y, r16(__fmul_rn(cs, __half2float(zh[e])))));
+      oh[e] = __float2half_rn(y);
+    }
     reinterpret_cast<uint4*>(out)[i] = ov;
   }
   // tail (n not a multiple of 8)
   const long long tail0 = nvec << 3;
-  for (long long i = tail0 + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride)
-    out[i] = __float2half_rn(ddim_one(__half2float(x[i]), __half2float(vn[i]), cfg ? __half2float(ve[i]) : 0.f, cfg,
-                                      g, ca, cb, cc, cd));
+  for (long long i = tail0 + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+    float y = ddim_one(__half2float(x[i]), __half2float(vn[i]), cfg ? __half2float(ve[i]) : 0.f, cfg, g, ca, cb, cc, cd);
+    if (kNoise) y = r16(__fadd_rn(y, r16(__fmul_rn(cs, __half2float(z[i])))));
+    out[i] = __float2half_rn(y);
+  }
+}
+
+unsigned ddim_blocks(long long n) {
+  const long long nvec = (n + 7) >> 3;
+  long long blocks = (nvec + 255) / 256;
+  const long long cap = static_cast<long long>(sm_count_cached()) * 8;
+  if (blocks > cap) blocks = cap;
+  if (blocks < 1) blocks = 1;
+  return static_cast<unsigned>(blocks);
 }
 
 int ddim_launch(const av2v_ddim_args* a, cudaStream_t stream) {
@@ -69,14 +90,25 @@ int ddim_launch(const av2v_ddim_args* a, cudaStream_t stream) {
   AV2V_REQUIRE(a->x && a->v_neg && a->out, AV2V_EINVAL, "ddim: null x / v_neg / out");
   AV2V_REQUIRE(aligned16(a->x) && aligned16(a->v_neg) && aligned16(a->out) && (!a->v_edit || aligned16(a->v_edit)),
                AV2V_EALIGN, "ddim: pointers must be 16-byte aligned");
-  const long long nvec = (a->n + 7) >> 3;
-  long long blocks = (nvec + 255) / 256;
-  const long long cap = static_cast<long long>(sm_count_cached()) * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  ddim_step_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
+  ddim_step_kernel<false><<<ddim_blocks(a->n), 256, 0, stream>>>(
       static_cast<const __half*>(a->x), static_cast<const __half*>(a->v_neg), static_cast<const __half*>(a->v_edit),
-      static_cast<__half*>(a->out), a->n, a->guidance, a->ca, a->cb, a->cc, a->cd, a->coef_dev);
+      nullptr, static_cast<__half*>(a->out), a->n, a->guidance, a->ca, a->cb, a->cc, a->cd, 0.f, a->coef_dev);
+  AV2V_CHECK_CUDA(cudaGetLastError());
+  return AV2V_OK;
+}
+
+int ddim_eta_launch(const av2v_ddim_eta_args* a, cudaStream_t stream) {
+  AV2V_REQUIRE(a != nullptr, AV2V_EINVAL, "ddim_eta: null args");
+  AV2V_REQUIRE(a->n >= 0, AV2V_EINVAL, "ddim_eta: negative element count");
+  if (a->n == 0) return AV2V_OK;
+  AV2V_REQUIRE(a->x && a->v_neg && a->noise && a->out, AV2V_EINVAL, "ddim_eta: null x / v_neg / noise / out");
+  AV2V_REQUIRE(aligned16(a->x) && aligned16(a->v_neg) && aligned16(a->noise) && aligned16(a->out) &&
+                   (!a->v_edit || aligned16(a->v_edit)),
+               AV2V_EALIGN, "ddim_eta: pointers must be 16-byte aligned");
+  ddim_step_kernel<true><<<ddim_blocks(a->n), 256, 0, stream>>>(
+      static_cast<const __half*>(a->x), static_cast<const __half*>(a->v_neg), static_cast<const __half*>(a->v_edit),
+      static_cast<const __half*>(a->noise), static_cast<__half*>(a->out), a->n, a->guidance, a->ca, a->cb, a->cc, a->cd,
+      a->cs, a->coef_dev);
   AV2V_CHECK_CUDA(cudaGetLastError());
   return AV2V_OK;
 }
@@ -301,4 +333,7 @@ extern "C" int av2v_ddim_step_cfg_f16(const av2v_ddim_args* a, av2v_stream_t str
 }
 extern "C" int av2v_ddim_inverse_step_f16(const av2v_ddim_args* a, av2v_stream_t stream) {
   return ddim_launch(a, static_cast<cudaStream_t>(stream));
+}
+extern "C" int av2v_ddim_step_eta_f16(const av2v_ddim_eta_args* a, av2v_stream_t stream) {
+  return ddim_eta_launch(a, static_cast<cudaStream_t>(stream));
 }

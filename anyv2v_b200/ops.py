@@ -144,6 +144,34 @@ def ddim_step(x, v_neg, v_edit, guidance: float, ca: float, cb: float, cc: float
     return out
 
 
+def ddim_step_eta(x, v_neg, v_edit, noise, guidance: float, ca: float, cb: float, cc: float, cd: float, cs: float, out=None,
+                  coef_dev=None):
+    """``ddim_step`` with DDIM's variance noise (eta > 0): out = fp16(update + fp16(cs * noise)), cd = sqrt(1 - a_prev - cs^2).
+    ``noise`` is in x's element order.  ``coef_dev``: device {ca, cb, cc, cd, guidance, cs}."""
+    global _launches
+    n = x.numel()
+    _vector(x, "ddim_step_eta.x", n)
+    _vector(v_neg, "ddim_step_eta.v_neg", n)
+    _vector(v_edit, "ddim_step_eta.v_edit", n)
+    _f16_cuda(noise, "ddim_step_eta.noise")
+    _require(noise.device == x.device, f"ddim_step_eta.noise: on {noise.device}, x on {x.device}")
+    _vector(noise, "ddim_step_eta.noise", n)
+    if out is None:
+        out = torch.empty_like(x)
+    _f16_cuda(out, "ddim_step_eta.out")
+    _require(out.device == x.device, f"ddim_step_eta.out: on {out.device}, x on {x.device}")
+    _vector(out, "ddim_step_eta.out", n)
+    if coef_dev is not None:
+        _require(coef_dev.device == x.device and coef_dev.dtype == torch.float32 and coef_dev.numel() >= 6,
+                 f"ddim_step_eta.coef_dev: expected >= 6 fp32 values on {x.device}, got {coef_dev.numel()} "
+                 f"{coef_dev.dtype} on {coef_dev.device}")
+    a = L.DdimEtaArgs(_p(x), _p(v_neg), _p(v_edit), _p(noise), _p(out), n, guidance, ca, cb, cc, cd, cs, _p(coef_dev))
+    with _timed("ddim_step_eta"):
+        L.check(L.lib().av2v_ddim_step_eta_f16(ctypes.byref(a), _stream()), "av2v_ddim_step_eta")
+    _launches += 1
+    return out
+
+
 # ----------------------------------------------------------------------------------------------------------- K6
 def groupnorm(x, gamma, beta, groups: int, eps: float, silu: bool, out=None, x2=None):
     """GroupNorm(+SiLU) over x[n_samples, rows, C] (channels-last). pnp_utils.py:48-49,92,104.

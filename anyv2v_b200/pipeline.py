@@ -1,8 +1,9 @@
-"""I2VGen-XL sampling loops, H100-native: ``invert`` and ``sample_with_pnp``.
+"""I2VGen-XL sampling loops, H100-native: ``invert``, ``sample_with_pnp`` and the image-to-video call ``pipe(...)``.
 
-Drop-in for the two hot loops of the reference's ``I2VGenXLPipeline`` (i2vgen-xl/pipelines/pipeline_i2vgen_xl.py):
+Drop-in for the hot loops of the reference's ``I2VGenXLPipeline`` (i2vgen-xl/pipelines/pipeline_i2vgen_xl.py):
   invert            :1197-1439 (loop :1385-1433)
   sample_with_pnp   :892-1195  (loop :1131-1179)
+  __call__          :652-890   (loop :839-874; also eta > 0)
 with the same keyword surface for everything that reaches the loops.  Differences, none of which changes a result:
   * no host sync inside the loop: timesteps are Python ints (the reference calls ``t.item()`` at :1143 and runs
     ``t in tensor`` membership kernels inside every hook), inverted latents stay in HBM (anyv2v_b200.latent_store)
@@ -27,6 +28,7 @@ import torch
 
 from .latent_store import LatentStore
 from .pnp_utils import _fires, register_time
+from .schedulers import randn_tensor
 
 logger = logging.getLogger(__name__)
 
@@ -211,6 +213,145 @@ class I2VGenXLPipeline:
                     if _fires(t, getattr(proc, "_injection_set", None)):
                         return True
         return False
+
+    # -- image-to-video sampling (pipeline :652-890) ------------------------------------------------------------------
+    @torch.no_grad()
+    def __call__(self, prompt=None, image=None, height: Optional[int] = 704, width: Optional[int] = 1280,
+                 target_fps: int = 16, num_frames: int = 16, num_inference_steps: int = 50, guidance_scale: float = 9.0,
+                 negative_prompt=None, eta: float = 0.0, num_videos_per_prompt: int = 1,
+                 decode_chunk_size: Optional[int] = 1, generator=None, latents: Optional[torch.Tensor] = None,
+                 prompt_embeds=None, negative_prompt_embeds=None, output_type: str = "pil", return_dict: bool = True,
+                 ddim_init_latents_t_idx: int = 1, image_embeddings=None, image_latents=None,
+                 callback: Optional[Callable] = None, max_steps: Optional[int] = None, **_ignored):
+        """Image-to-video DDIM sampling with CFG (pipeline :652-890), the reference's keyword surface and defaults.  Note the
+        reference's ``ddim_init_latents_t_idx=1``: the first timestep is skipped (:812-813).  ``eta > 0`` samples
+        stochastically, drawing sigma_t * z from ``generator`` at every step as diffusers' DDIMScheduler does.  Raw inputs
+        (``prompt`` strings, PIL ``image``) need ``encoders=`` and ``vae=``; pre-encoded ``prompt_embeds`` /
+        ``negative_prompt_embeds`` / ``image_embeddings`` / ``image_latents`` (batch 1) are accepted instead.
+        ``output_type`` "latent" returns the latents [N, 4, F, h, w]; "pt" / "np" / "pil" decode them with the attached VAE."""
+        if isinstance(prompt, list):
+            if len(prompt) != 1:  # the reference builds its image latents per video, not per prompt (:797-802)
+                raise ValueError(f"one prompt per call (got {len(prompt)}): use num_videos_per_prompt for several videos")
+            prompt = prompt[0]
+        if isinstance(negative_prompt, list):
+            if len(negative_prompt) != 1:
+                raise ValueError(f"one negative prompt per call (got {len(negative_prompt)})")
+            negative_prompt = negative_prompt[0]
+        if height is None or width is None:
+            height, width = self._size_of(image, height, width)
+        if height is not None and width is not None and (height % 8 != 0 or width % 8 != 0):
+            raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
+        n_videos = int(num_videos_per_prompt)
+        if isinstance(generator, list):
+            if len(generator) != n_videos:
+                raise ValueError(f"You have passed a list of generators of length {len(generator)}, but requested an effective "
+                                 f"batch size of {n_videos}. Make sure the batch size matches the length of the generators.")
+            if eta > 0 and len(generator) > 1:  # the reference's step noise would index the list per frame (:868)
+                raise ValueError("eta > 0 draws the step noise from one generator: pass a single torch.Generator")
+        self._guidance_scale = guidance_scale
+        if prompt_embeds is None and prompt is not None:
+            prompt_embeds = self.encode_prompt(prompt)
+        if (self.do_classifier_free_guidance and negative_prompt_embeds is None
+                and (negative_prompt is not None or prompt is not None)):
+            negative_prompt_embeds = self.encode_prompt(negative_prompt if negative_prompt is not None else "")
+        if image is not None and (image_embeddings is None or image_latents is None):
+            # the reference samples the first-frame latent with the global RNG (:540 passes no generator)
+            emb, lat = self.encode_first_frame(image, height, width, num_frames, generator=None)
+            image_embeddings = emb if image_embeddings is None else image_embeddings
+            image_latents = lat if image_latents is None else image_latents
+        if latents is None and prompt_embeds is not None and image_latents is not None:  # prepare_latents :595-621
+            shape = (n_videos, self.unet.config["in_channels"], num_frames) + tuple(image_latents.shape[-2:])
+            latents = randn_tensor(shape, generator=generator, device=self.device, dtype=prompt_embeds.dtype)
+        st = self.prepare_call(latents, prompt_embeds, image_latents, image_embeddings, target_fps, num_inference_steps,
+                               guidance_scale, negative_prompt_embeds, eta, generator, ddim_init_latents_t_idx)
+        n = len(st.timesteps) if max_steps is None else min(max_steps, len(st.timesteps))
+        for i in range(n):
+            self.call_step(st, i)
+            if callback is not None:
+                callback(i, st.timesteps[i], st.latents)
+        if output_type == "latent":
+            return SimpleNamespace(frames=st.latents) if return_dict else (st.latents,)
+        video = tensor2vid(self.decode_latents(st.latents, decode_chunk_size=decode_chunk_size), output_type)
+        return SimpleNamespace(frames=video) if return_dict else (video,)
+
+    def prepare_call(self, latents, prompt_embeds, image_latents, image_embeddings, target_fps=16, num_inference_steps=50,
+                     guidance_scale=9.0, negative_prompt_embeds=None, eta=0.0, generator=None, ddim_init_latents_t_idx=1):
+        """Everything of ``__call__`` that happens once per clip (pipeline :742-834): ``latents`` [N, 4, F, h, w] and the
+        conditioning of one prompt / first frame (batch 1), repeated for the N videos.  With CFG the UNet batch is
+        [uncond x N, cond x N] (:783, :437-439, :559-560)."""
+        self._guidance_scale = guidance_scale
+        self.check_inputs(prompt_embeds, image_latents, image_embeddings, latents)
+        cfg = self.do_classifier_free_guidance
+        if cfg and negative_prompt_embeds is None:
+            raise ValueError("`negative_prompt_embeds` (or a `negative_prompt` string + encoders) is required when guidance_scale > 1")
+        if eta < 0:
+            raise ValueError(f"eta must be >= 0, got {eta}")
+        for name, t in (("prompt_embeds", prompt_embeds), ("negative_prompt_embeds", negative_prompt_embeds),
+                        ("image_embeddings", image_embeddings), ("image_latents", image_latents)):
+            if t is not None and t.shape[0] != 1:
+                raise ValueError(f"`{name}` must hold one prompt / first frame (batch 1), got {tuple(t.shape)}: "
+                                 "num_videos_per_prompt repeats it")
+        dev = self.device
+        n_videos = latents.shape[0]
+        rep = lambda x: x.to(dev).repeat(n_videos, *([1] * (x.dim() - 1)))
+        if cfg:
+            prompts = torch.cat([rep(negative_prompt_embeds), rep(prompt_embeds)])
+            img_emb = torch.cat([torch.zeros_like(rep(image_embeddings)), rep(image_embeddings)])
+            img_lat = torch.cat([rep(image_latents)] * 2)
+        else:
+            prompts, img_emb, img_lat = rep(prompt_embeds), rep(image_embeddings), rep(image_latents)
+        fps = torch.tensor([target_fps] * img_lat.shape[0], device=dev)
+        cond = self.unet.precompute_conditioning(fps, img_lat, img_emb, prompts)
+        self.scheduler.set_timesteps(num_inference_steps, device=dev)
+        self.scheduler.timesteps = self.scheduler.timesteps[ddim_init_latents_t_idx:]
+        ts = self.scheduler.timesteps.tolist()
+        logger.info("Sampling starts from latents_at_t=%s", ts[0] if ts else None)
+        st = SimpleNamespace(latents=latents.to(dev).contiguous().clone(), cond=cond, timesteps=ts, eta=float(eta),
+                             generator=generator, scheduler=self.scheduler, n_videos=n_videos)
+        st.t_table = torch.tensor(ts, device=dev, dtype=torch.int64)
+        st.coef_table = self.scheduler.coefficient_table(ts, guidance_scale if cfg else 1.0, dev, eta=st.eta)
+        st.g_t = torch.zeros(1, device=dev, dtype=torch.int64)
+        st.g_coef = torch.zeros(st.coef_table.shape[1], device=dev, dtype=torch.float32)
+        st.g_noise = torch.zeros_like(st.latents) if st.eta > 0 else None
+        # uncond and cond of one video have the same latents, image latents, fps and timestep: they share the UNet prefix
+        # up to the first cross-attention.  With N > 1 the last two branches are different videos.
+        st.shared_prefix = cfg and n_videos == 1
+
+        if cfg:
+            def body():
+                v = self.unet(torch.cat([st.latents, st.latents]), st.g_t, cond=st.cond, shared_edit_prefix=st.shared_prefix)[0]
+                st.scheduler.step(v[:n_videos], None, st.latents, eta=st.eta, model_output_cond=v[n_videos:], out=st.latents,
+                                  coef_dev=st.g_coef, variance_noise=st.g_noise)
+        else:
+            def body():
+                v = self.unet(st.latents, st.g_t, cond=st.cond)[0]
+                st.scheduler.step(v, None, st.latents, eta=st.eta, out=st.latents, coef_dev=st.g_coef,
+                                  variance_noise=st.g_noise)
+
+        st.body = body
+        st.iterations = {}  # (FreeU setting, eta > 0) -> _GraphedIteration
+        st.graph_pool = torch.cuda.graph_pool_handle() if st.latents.is_cuda else None
+        return st
+
+    def call_step(self, st, i: int):
+        """One iteration of the sampling loop (pipeline :839-874): UNet on [uncond, cond] -> CFG + DDIM step, in place.
+        With eta > 0 the step noise is drawn here, eagerly and in the reference's [N*F, C, h, w] order (:864-868), so that
+        the draws from ``generator`` are those of the reference, and copied into the buffer the (captured) step reads."""
+        if st.g_noise is not None:
+            n, c, f, h, w = st.latents.shape
+            z = randn_tensor((n * f, c, h, w), generator=st.generator, device=st.latents.device, dtype=st.latents.dtype)
+            st.g_noise.copy_(z.view(n, f, c, h, w).permute(0, 2, 1, 3, 4))
+        st.g_t.copy_(st.t_table[i:i + 1])
+        st.g_coef.copy_(st.coef_table[i])
+        key = (self.unet.freeu_state(), st.eta > 0)
+        it = st.iterations.get(key)
+        if it is None:
+            it = st.iterations[key] = _GraphedIteration(st.body, on_cuda=st.latents.is_cuda, pool=st.graph_pool)
+        if self.use_cuda_graphs:
+            it.run()
+        else:
+            it.body()
+        return st.latents
 
     # -- phase 1 --------------------------------------------------------------------------------------------------
     @torch.no_grad()

@@ -48,20 +48,24 @@ def ddim_inversion(config, first_frame, frame_list, pipe: I2VGenXLPipeline, inve
 
 
 def ddim_sampling(config, first_frame, ddim_latents_path, pipe, ddim_scheduler, ddim_init_latents_t_idx, g, cond=None):
-    """reference :58-77 (DDIM reconstruction, the authors' sanity check): plain CFG sampling from x_t without hooks."""
+    """reference :58-77 (DDIM reconstruction, the authors' sanity check): ``pipe(...)`` from x_t, without hooks.  Returns the
+    reconstructed latents [1, 4, F, h, w]; with PIL ``first_frame`` (real inputs) also the decoded frames, else None."""
     from .latent_store import load_ddim_latents_at_t
     ddim_scheduler.set_timesteps(config.n_steps)
-    ts = ddim_scheduler.timesteps.tolist()[ddim_init_latents_t_idx:]
-    latents = load_ddim_latents_at_t(ts[0], ddim_latents_path, map_location=pipe.device)
-    dev = pipe.device
-    prompts = torch.cat([cond["neg_prompt"], cond["inv_prompt"]])
-    img_emb = torch.cat([torch.zeros_like(cond["src_image_emb"]), cond["src_image_emb"]])
-    img_lat = torch.cat([cond["src_image_latents"]] * 2)
-    c2 = pipe.unet.precompute_conditioning(torch.tensor([config.target_fps] * 2, device=dev), img_lat, img_emb, prompts)
-    for t in ts:
-        v = pipe.unet(torch.cat([latents, latents]), torch.tensor([t], device=dev), cond=c2)[0]
-        latents = ddim_scheduler.step(v[0:1], t, latents, model_output_cond=v[1:2], guidance_scale=config.cfg).prev_sample
-    return latents
+    t0 = ddim_scheduler.timesteps.tolist()[ddim_init_latents_t_idx]
+    latents = load_ddim_latents_at_t(t0, ddim_latents_path, map_location=pipe.device)
+    pipe.scheduler = ddim_scheduler
+    common = dict(num_frames=config.n_frames, num_inference_steps=config.n_steps, guidance_scale=config.cfg,
+                  target_fps=config.target_fps, latents=latents, generator=g, ddim_init_latents_t_idx=ddim_init_latents_t_idx,
+                  output_type="latent", return_dict=True)
+    if cond is not None:  # synthetic opt-in: pre-encoded conditioning
+        rec = pipe(prompt_embeds=cond["inv_prompt"], negative_prompt_embeds=cond["neg_prompt"],
+                   image_embeddings=cond["src_image_emb"], image_latents=cond["src_image_latents"], **common).frames
+        return rec, None
+    from .pipeline import tensor2vid
+    rec = pipe(prompt=config.prompt, image=first_frame, height=int(config.image_size[1]), width=int(config.image_size[0]),
+               negative_prompt=config.negative_prompt, **common).frames
+    return rec, tensor2vid(pipe.decode_latents(rec, decode_chunk_size=1), "pil")[0]
 
 
 def main(template_config, configs_list, device, unet_config=None, pipeline_kwargs=None):
@@ -112,13 +116,18 @@ def main(template_config, configs_list, device, unet_config=None, pipeline_kwarg
         out.append(inv)
         rc = config.recon_config
         if rc.enable_recon:
-            if cond is None:  # real inputs: encode what the reconstruction's plain CFG sampling needs (reference :58-77)
-                emb, lat = pipe.encode_first_frame(first_frame, int(config.image_size[1]), int(config.image_size[0]), config.n_frames)
-                cond = {"neg_prompt": pipe.encode_prompt(rc.negative_prompt), "inv_prompt": pipe.encode_prompt(rc.prompt),
-                        "src_image_emb": emb, "src_image_latents": lat}
-            rec = ddim_sampling(rc, None, rc.ddim_latents_path, pipe, ddim_scheduler, rc.ddim_init_latents_t_idx, g, cond=cond)
+            rec, frames = ddim_sampling(rc, None if cond is not None else first_frame, rc.ddim_latents_path, pipe,
+                                        ddim_scheduler, rc.ddim_init_latents_t_idx, g, cond=cond)
             os.makedirs(os.path.join(config.output_dir, "ddim_reconstruction"), exist_ok=True)
             torch.save(rec.cpu(), os.path.join(config.output_dir, "ddim_reconstruction", "latents.pt"))
+            if frames is not None:  # reference :180-192: down-sampled for space, mp4 at 10 fps + gif
+                from PIL import Image
+
+                from . import image_io
+                frames = [f.resize((512, 512), resample=Image.LANCZOS) for f in frames]
+                image_io.export_to_video(frames, os.path.join(config.output_dir, "ddim_reconstruction.mp4"), fps=10)
+                image_io.export_to_gif(frames, os.path.join(config.output_dir, "ddim_reconstruction.gif"))
+                logger.info("Saved reconstructed video to %s", config.output_dir)
     return out
 
 

@@ -38,6 +38,28 @@ def _alphas_cumprod(cfg) -> torch.Tensor:
     return torch.cumprod(1.0 - betas, dim=0)
 
 
+def randn_tensor(shape, generator=None, device=None, dtype=None):
+    """diffusers.utils.torch_utils.randn_tensor [recalled]: a CPU generator draws on the CPU (in ``dtype``) and the result is
+    moved to ``device``; a CUDA generator for a CPU tensor is an error; a list of generators draws one batch entry each (a
+    list of one is a single generator)."""
+    device = torch.device(device) if device is not None else torch.device("cpu")
+    rand_device = device
+    batch_size = shape[0]
+    if generator is not None:
+        gen_device_type = generator.device.type if not isinstance(generator, list) else generator[0].device.type
+        if gen_device_type != device.type and gen_device_type == "cpu":
+            rand_device = "cpu"
+        elif gen_device_type != device.type and gen_device_type == "cuda":
+            raise ValueError(f"Cannot generate a {device} tensor from a generator of type {gen_device_type}.")
+    if isinstance(generator, list) and len(generator) == 1:
+        generator = generator[0]
+    if isinstance(generator, list):
+        shape = (1,) + tuple(shape[1:])
+        latents = [torch.randn(shape, generator=generator[i], device=rand_device, dtype=dtype) for i in range(batch_size)]
+        return torch.cat(latents, dim=0).to(device)
+    return torch.randn(tuple(shape), generator=generator, device=rand_device, dtype=dtype).to(device)
+
+
 class _DDIMBase:
     order = 1
     init_noise_sigma = 1.0
@@ -75,32 +97,62 @@ class _DDIMBase:
     def _alpha_pair(self, timestep):
         raise NotImplementedError
 
-    def coefficients(self, timestep):
+    def coefficients(self, timestep, eta: float = 0.0):
         """(sqrt(a_in), sqrt(1-a_in), sqrt(a_out), sqrt(1-a_out)) as Python floats holding exact fp32 values,
-        computed with the same fp32 torch ops as the reference (`alpha ** 0.5`)."""
+        computed with the same fp32 torch ops as the reference (`alpha ** 0.5`).  With ``eta > 0`` (DDIMScheduler only):
+        (ca, cb, cc, cd', cs) with cs = sigma_t = eta * sqrt(variance) and cd' = sqrt(1 - a_out - sigma_t^2), the fp32 0-dim
+        torch ops of diffusers' `DDIMScheduler._get_variance` / `step` [recalled: diffusers is not vendored]."""
         a_in, a_out = self._alpha_pair(int(timestep))
-        return tuple(float(c) for c in (a_in ** 0.5, (1 - a_in) ** 0.5, a_out ** 0.5, (1 - a_out) ** 0.5))
+        if eta == 0.0:
+            return tuple(float(c) for c in (a_in ** 0.5, (1 - a_in) ** 0.5, a_out ** 0.5, (1 - a_out) ** 0.5))
+        std_dev_t = eta * self._variance(a_in, a_out) ** (0.5)
+        return tuple(float(c) for c in (a_in ** 0.5, (1 - a_in) ** 0.5, a_out ** 0.5, (1 - a_out - std_dev_t ** 2) ** (0.5),
+                                        std_dev_t))
+
+    def _variance(self, a_in, a_out):
+        raise ValueError(f"{type(self).__name__}.step has no eta (consisti2v/ddim_inverse_scheduler.py:291-297)")
 
     def step(self, model_output, timestep, sample, eta: float = 0.0, return_dict: bool = True, *,
-             model_output_cond=None, guidance_scale: float = 1.0, out=None, coef_dev=None, **_unused):
+             model_output_cond=None, guidance_scale: float = 1.0, out=None, coef_dev=None, generator=None,
+             variance_noise=None, **_unused):
         """x_t -> x_{t-1} (DDIM) or x_t -> x_{t+1} (inverse).  With ``model_output_cond`` the CFG combine
-        ``uncond + g*(cond-uncond)`` (pipeline :1162) is fused into the same launch."""
-        if eta != 0.0:
-            raise ValueError("the AnyV2V path samples with eta = 0")
-        ca, cb, cc, cd = (0.0, 0.0, 0.0, 0.0) if coef_dev is not None else self.coefficients(timestep)
-        prev = ops.ddim_step(sample.contiguous(), model_output.contiguous(),
-                             None if model_output_cond is None else model_output_cond.contiguous(),
-                             float(guidance_scale), ca, cb, cc, cd, out=out, inverse=self._inverse, coef_dev=coef_dev)
+        ``uncond + g*(cond-uncond)`` (pipeline :1162) is fused into the same launch.  ``eta > 0`` (DDIMScheduler) adds
+        sigma_t * variance_noise in the same launch; the noise is drawn in ``model_output.shape`` from ``generator`` unless
+        ``variance_noise`` is given (diffusers' rule [recalled]: not both)."""
+        if eta < 0.0:
+            raise ValueError(f"eta must be >= 0, got {eta}")
+        if eta == 0.0:
+            ca, cb, cc, cd = (0.0, 0.0, 0.0, 0.0) if coef_dev is not None else self.coefficients(timestep)
+            prev = ops.ddim_step(sample.contiguous(), model_output.contiguous(),
+                                 None if model_output_cond is None else model_output_cond.contiguous(),
+                                 float(guidance_scale), ca, cb, cc, cd, out=out, inverse=self._inverse, coef_dev=coef_dev)
+        else:
+            if self._inverse:
+                self._variance(None, None)
+            if generator is not None and variance_noise is not None:
+                raise ValueError("Cannot pass both generator and variance_noise. Please make sure that either `generator` or"
+                                 " `variance_noise` stays `None`.")
+            if variance_noise is None:
+                variance_noise = randn_tensor(model_output.shape, generator=generator, device=model_output.device,
+                                              dtype=model_output.dtype)
+            ca, cb, cc, cd, cs = (0.0,) * 5 if coef_dev is not None else self.coefficients(timestep, eta)
+            prev = ops.ddim_step_eta(sample.contiguous(), model_output.contiguous(),
+                                     None if model_output_cond is None else model_output_cond.contiguous(),
+                                     variance_noise.contiguous(), float(guidance_scale), ca, cb, cc, cd, cs, out=out,
+                                     coef_dev=coef_dev)
         prev = prev.view(sample.shape)
         if not return_dict:
             return (prev,)
         return SimpleNamespace(prev_sample=prev)
 
-
-    def coefficient_table(self, timesteps, guidance_scale: float, device) -> torch.Tensor:
+    def coefficient_table(self, timesteps, guidance_scale: float, device, eta: float = 0.0) -> torch.Tensor:
         """[len(timesteps), 5] fp32 device table {ca, cb, cc, cd, guidance}: the per-step scalars of ``step`` as DATA,
-        so a captured CUDA graph of one loop iteration can be replayed for every timestep."""
-        rows = [list(self.coefficients(t)) + [float(guidance_scale)] for t in timesteps]
+        so a captured CUDA graph of one loop iteration can be replayed for every timestep.  ``eta > 0``: [len, 6]
+        {ca, cb, cc, cd', guidance, cs}, the ``coef_dev`` layout of ``ops.ddim_step_eta``."""
+        rows = []
+        for t in timesteps:
+            c = list(self.coefficients(t, eta))
+            rows.append(c[:4] + [float(guidance_scale)] + c[4:])
         return torch.tensor(rows, dtype=torch.float32).to(device)
 
 
@@ -116,6 +168,13 @@ class DDIMScheduler(_DDIMBase):
         t_prev = t - self.config.num_train_timesteps // self.num_inference_steps
         a_prev = self.alphas_cumprod[t_prev] if t_prev >= 0 else self.final_alpha_cumprod
         return self.alphas_cumprod[t], a_prev
+
+    def _variance(self, alpha_prod_t, alpha_prod_t_prev):
+        """diffusers `DDIMScheduler._get_variance` [recalled], fp32 0-dim tensors; the same sigma as
+        seine/diffusion/gaussian_diffusion.py:585-589"""
+        beta_prod_t = 1 - alpha_prod_t
+        beta_prod_t_prev = 1 - alpha_prod_t_prev
+        return (beta_prod_t_prev / beta_prod_t) * (1 - alpha_prod_t / alpha_prod_t_prev)
 
 
 class DDIMInverseScheduler(_DDIMBase):

@@ -40,7 +40,7 @@ const char* av2v_last_error(void); /* thread-local, valid until the next failing
 int av2v_device_info(int* sm_count, int* cc_major, int* cc_minor);
 
 /* ------------------------------------------------------------------------------------------------------------
- * K7  CFG combine + DDIM step (v-prediction, eta = 0) and its inverse.
+ * K7  CFG combine + DDIM step (v-prediction; eta = 0, and eta > 0 with variance noise) and its inverse.
  * Replaces: pipeline_i2vgen_xl.py:1159-1176 (CFG, reshape, scheduler.step) and :1407-1420 (inversion), with
  * diffusers DDIMScheduler.step / DDIMInverseScheduler.step (vendored twin consisti2v/ddim_inverse_scheduler.py:329-369).
  * Reproduces the reference's rounding sequence: every product / sum is computed in fp32 and rounded to fp16
@@ -64,6 +64,24 @@ typedef struct {
 } av2v_ddim_args;
 int av2v_ddim_step_cfg_f16(const av2v_ddim_args* a, av2v_stream_t stream);
 int av2v_ddim_inverse_step_f16(const av2v_ddim_args* a, av2v_stream_t stream);
+
+/* Stochastic DDIM (eta > 0; pipeline_i2vgen_xl.py:834,868 forward eta and generator to diffusers DDIMScheduler.step),
+ * the same kernel with the variance noise added as two more separately rounded ops:
+ *   out = r16( ddim(x, v_neg, v_edit; ca, cb, cc, cd) + r16(cs * noise) )
+ * with  var = (1 - a_prev)/(1 - a_t) * (1 - a_t/a_prev),  cs = sigma = eta * sqrt(var),  cd = sqrt(1 - a_prev - cs^2)
+ * (ca, cb, cc as above).  noise is in the element order of x (the kernel is elementwise). */
+typedef struct {
+  const void* x;      /* current latents, n fp16 */
+  const void* v_neg;  /* model output (uncond chunk when CFG is on), n fp16 */
+  const void* v_edit; /* cond chunk, or NULL for no CFG */
+  const void* noise;  /* standard-normal draw z, n fp16 */
+  void* out;          /* n fp16; may alias x */
+  int64_t n;
+  float guidance;
+  float ca, cb, cc, cd, cs;
+  const float* coef_dev; /* optional device pointer to {ca, cb, cc, cd, guidance, cs}, read INSTEAD of the by-value fields */
+} av2v_ddim_eta_args;
+int av2v_ddim_step_eta_f16(const av2v_ddim_eta_args* a, av2v_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * K6  GroupNorm (+ optional SiLU), channels-last.
