@@ -49,20 +49,23 @@ struct GemmP {
   int n_tiles, num_kb;
 };
 
-// Exact-erf GELU, branch-free: gelu(g) = g/2 + |g|/2 * erf(|g|/sqrt 2) with erf from Abramowitz & Stegun 7.1.25
-// (3-term, |abs err| < 2.5e-5 — two orders below fp16 resolution) on MUFU rcp / ex2: ~14 instructions per element;
-// libdevice erff costs about twice as much and diverges.
+// Exact-erf GELU, branch-free: gelu(g) = g/2 * erfc(-g/sqrt 2).  With E = erfc(z), z = |g|/sqrt 2:
+//   g < 0: gelu = g/2 * E;   g >= 0: gelu = g - g/2 * E   ->   gelu = max(g, 0) - |g/2| * E.
+// E has the form of the erfcc routine of Numerical Recipes, t = 1 / (1 + z/2), E = t * exp(-z^2 + P(t)), with a degree-5 P
+// fitted in tools/erfc_poly_fit.py: its error is RELATIVE (< 1.4e-5 on z in [0, 5.6], fp32 evaluation included), so the
+// small negative-gate side keeps full fp16 precision.  (An absolute-error erf — A&S 7.1.25, 2.5e-5 — was 20 fp16 ulps off at
+// gates in [-4, -3], where gelu is ~1e-3.)  MUFU rcp + ex2 and ~9 FMAs per element; libdevice erfcf costs more and diverges.
 __device__ __forceinline__ float gelu_erf_fast(float g) {
-  const float u = fabsf(g) * 0.70710678118654752f;
+  const float z = fabsf(g) * 0.70710678118654752f;
   float t;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(fmaf(0.47047f, u, 1.0f)));
-  float poly = fmaf(t, 0.7478556f, -0.0958798f);
-  poly = fmaf(poly, t, 0.3480242f);
-  poly *= t;
-  const float e = ex2_approx(u * u * -1.4426950408889634f);
-  const float erf_abs = fmaf(-poly, e, 1.0f);
-  const float hg = 0.5f * g;
-  return fmaf(fabsf(hg), erf_abs, hg);
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(fmaf(0.5f, z, 1.0f)));
+  float p = fmaf(t, 0.22427836f, -0.69402432f);
+  p = fmaf(p, t, 0.45475456f);
+  p = fmaf(p, t, 0.26681793f);
+  p = fmaf(p, t, 1.01429605f);
+  p = fmaf(p, t, -1.26611602f);
+  const float e = t * ex2_approx(fmaf(-z, z, p) * 1.4426950408889634f);
+  return fmaf(-fabsf(0.5f * g), e, fmaxf(g, 0.0f));
 }
 
 // Per-thread view of the A rows it gathers (rows r0 + 32 i, i = 0..3, of the tile): what the K loop needs to address them.

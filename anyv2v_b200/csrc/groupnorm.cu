@@ -13,7 +13,8 @@
 //   * rows are contiguous in the channels-last layout, so a slice of rows is ONE byte range: a producer warp moves it with
 //     1-D bulk TMA copies (cp.async.bulk, kStages x ~20 KB in flight per SM, completion on mbarriers); the consumer threads
 //     only ever read shared memory.  No per-thread global loads, no address arithmetic in the inner loop.
-//   * deterministic: per-(sample, slice, group) partial sums in a fixed order, folded in double; no float atomics.
+//   * deterministic: per-(sample, slice, group) partial sums of x - k (k: one pivot element per sample and group, so the
+//     variance does not cancel when |mean| >> sigma) in a fixed order, folded in double; no float atomics.
 //     The grid barrier is one integer atomic per CTA and chunk.
 #include "host_util.cuh"
 #include "ptx.cuh"
@@ -74,6 +75,14 @@ __device__ __forceinline__ void mbar_wait_hot(uint64_t* bar, uint32_t parity) {
       __trap();
     }
   }
+}
+
+// the statistics pivot of (sample s, group g): the group's first channel in row 0 of the sample, read from the source that holds
+// it (so the two-source form and the concatenated input shift by the same value)
+__device__ __forceinline__ __half gn_pivot(const GnParams& p, int s, int g) {
+  const int c = g * p.cpg;
+  const long long row0 = static_cast<long long>(s) * p.rows;
+  return c < p.C1 ? p.x[row0 * p.C1 + c] : p.x2[row0 * (p.C - p.C1) + (c - p.C1)];
 }
 
 template <int U, int kMaxT>
@@ -179,8 +188,14 @@ gn_persistent_kernel(const GnParams p) {
     // A CTA's items j = b, b + G, ... of a chunk are in ascending sample order, so its items of one sample are consecutive: the
     // per-thread sums run across them and are folded ONCE per (CTA, sample) into partial[sample][slot], slot = offset of the CTA's
     // first item inside the sample = a number in [0, min(slices, G)) that exactly one CTA owns (no zero-fill, no atomics).
+    // The sums are SHIFTED: S1 = sum (x - k), S2 = sum (x - k)^2 with one pivot k per (sample, group), the group's first channel
+    // in row 0 of the sample (gn_pivot).  Unshifted fp32 sums of x and x^2 lose the variance to cancellation in E[x^2] - mean^2
+    // once |mean| / sigma is large (at 300, 43 % of the outputs of a 64 x 64 frame were > 1 fp16 ulp off); x - k is of the size of
+    // sigma, so S2 / N - (S1 / N)^2 keeps the fp32 sums' relative precision.
     {
       float2 sm_[4], sq_[4];  // packed fp32x2 accumulators (two channels per issue slot; the same IEEE add / fma per lane)
+      uint4 kh = make_uint4(0u, 0u, 0u, 0u);  // pivots of this thread's 8 channels (fp16), for the sample being summed
+      int piv_sample = -1;
 #pragma unroll
       for (int e = 0; e < 4; ++e) sm_[e] = sq_[e] = make_float2(0.f, 0.f);
       int soff[U];  // this thread's vectors inside a stage (constant)
@@ -190,6 +205,12 @@ gn_persistent_kernel(const GnParams p) {
         const int j = static_cast<int>(blockIdx.x) + ii * G;
         const int sl_ = j / p.slices;  // sample index inside the chunk
         const int s = s0 + sl_, slice = j - sl_ * p.slices;
+        if (s != piv_sample) {
+          piv_sample = s;
+          __half* khh = reinterpret_cast<__half*>(&kh);
+#pragma unroll
+          for (int e = 0; e < 8; ++e) khh[e] = gn_pivot(p, s, (v * 8 + e) / p.cpg);
+        }
         int rbeg, rend;
         item_rows(slice, rbeg, rend);
         for (int r = rbeg; r < rend; r += p.stage_rows) {
@@ -198,16 +219,20 @@ gn_persistent_kernel(const GnParams p) {
           const uint4* sb = reinterpret_cast<const uint4*>(stage_buf + stage * kStageBytes + sbase);
           uint4 a4[U];
 #pragma unroll
-          for (int u = 0; u < U; ++u)
-            a4[u] = (r0 + u * p.rp < nr) ? sb[soff[u]] : make_uint4(0u, 0u, 0u, 0u);  // zeros add nothing to either sum
+          for (int u = 0; u < U; ++u) a4[u] = (r0 + u * p.rp < nr) ? sb[soff[u]] : kh;  // fill: x - k = 0 adds nothing
+          float2 kv[4];  // fp32 pivots, converted per stage (kept live across the loop they spill the 672-thread build)
+          const __half2* k2 = reinterpret_cast<const __half2*>(&kh);
+#pragma unroll
+          for (int e = 0; e < 4; ++e) kv[e] = __half22float2(k2[e]);
 #pragma unroll
           for (int u = 0; u < U; ++u) {
             const __half2* ah = reinterpret_cast<const __half2*>(&a4[u]);
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
               const float2 f = __half22float2(ah[e]);
-              sm_[e] = fadd2(sm_[e], f);
-              sq_[e] = ffma2(f, f, sq_[e]);
+              const float2 d = make_float2(__fsub_rn(f.x, kv[e].x), __fsub_rn(f.y, kv[e].y));
+              sm_[e] = fadd2(sm_[e], d);
+              sq_[e] = ffma2(d, d, sq_[e]);
             }
           }
           release_stage();
@@ -293,6 +318,7 @@ gn_persistent_kernel(const GnParams p) {
           const int subsets = T / p.groups;                // T is a multiple of 32 >= groups (groups <= 64 divides T for 32 / 64)
           const int g = t % p.groups, q = t / p.groups;
           const float2* src = reinterpret_cast<const float2*>(p.partial) + static_cast<long long>(s) * p.slots * p.groups + g;
+          const __half pivot = t < p.groups ? gn_pivot(p, s, t) : __float2half(0.f);  // in flight with the partial loads
           double ss = 0.0, qq = 0.0;
           if (q < subsets) {
             for (int sl = q; sl < p.slots; sl += 8 * subsets) {
@@ -320,8 +346,9 @@ gn_persistent_kernel(const GnParams p) {
               qq += dred[(k2 * p.groups + t) * 2 + 1];
             }
             const double cnt = static_cast<double>(p.rows) * p.cpg;
-            const double mean = ss / cnt;
-            double var = qq / cnt - mean * mean;
+            const double d1 = ss / cnt;  // mean of x - k
+            const double mean = static_cast<double>(__half2float(pivot)) + d1;
+            double var = qq / cnt - d1 * d1;
             if (var < 0.0) var = 0.0;
             stat[2 * t] = static_cast<float>(mean);
             stat[2 * t + 1] = static_cast<float>(1.0 / sqrt(var + static_cast<double>(p.eps)));

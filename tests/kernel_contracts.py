@@ -64,6 +64,13 @@ def ddim_step(x, v_neg, v_edit, guidance, ca, cb, cc, cd, out=None, inverse=Fals
 
 # ------------------------------------------------------------------------------------------------------------- K6
 def groupnorm(x, gamma, beta, groups, eps, silu, out=None, x2=None):
+    y = groupnorm_exact(x, gamma, beta, groups, eps, silu, x2=x2)
+    _count(1)
+    return _store(out, y, y.shape)
+
+
+def groupnorm_exact(x, gamma, beta, groups, eps, silu, x2=None):
+    """the float64 value ``groupnorm`` rounds to fp16 at the store, [n, rows, C]"""
     _f16(x, "groupnorm.x")
     assert x.dim() == 3 and x.is_contiguous()
     if x2 is not None:  # two-source input: the logical tensor is [x | x2] along the channels
@@ -78,16 +85,19 @@ def groupnorm(x, gamma, beta, groups, eps, silu, out=None, x2=None):
     if silu:
         y = y.to(torch.float16).double()  # the reference rounds the GroupNorm output before SiLU (two ops)
         y = y * torch.sigmoid(y)
-    _count(1)
-    return _store(out, y, x.shape)
+    return y.view(x.shape)
 
 
 def layernorm(x, gamma, beta, eps=1e-5, out=None):
-    _f16(x, "layernorm.x")
-    assert x.is_contiguous()
-    y = F.layer_norm(x.double(), (x.shape[-1],), gamma.double(), beta.double(), eps)
+    y = layernorm_exact(x, gamma, beta, eps)
     _count()
     return _store(out, y, x.shape)
+
+
+def layernorm_exact(x, gamma, beta, eps=1e-5):
+    _f16(x, "layernorm.x")
+    assert x.is_contiguous()
+    return F.layer_norm(x.double(), (x.shape[-1],), gamma.double(), beta.double(), eps)
 
 
 # ------------------------------------------------------------------------------------------------------------- GEMM
@@ -112,6 +122,17 @@ def _epilogue(y, bias, rowbias, rows_per_rowbias, residual2d):
 
 
 def linear(a, w, bias=None, residual=None, out=None, rowbias=None, rows_per_rowbias=0, geglu=False, a2=None):
+    y = linear_exact(a, w, bias, residual, rowbias, rows_per_rowbias, geglu, a2)
+    _count()
+    if out is None:
+        return y.to(torch.float16).contiguous()
+    assert out.stride(1) == 1
+    out.copy_(y.to(torch.float16))
+    return out
+
+
+def linear_exact(a, w, bias=None, residual=None, rowbias=None, rows_per_rowbias=0, geglu=False, a2=None):
+    """the float64 value ``linear`` rounds to fp16 at the store, [M, N] (GEGLU: [M, N / 2])"""
     _f16(a, "linear.a")
     if a2 is not None:  # two-source K loop: the logical A is [a | a2]
         _f16(a2, "linear.a2")
@@ -126,26 +147,13 @@ def linear(a, w, bias=None, residual=None, out=None, rowbias=None, rows_per_rowb
         y = (y[:, :, 0] * F.gelu(y[:, :, 1])).reshape(M, N // 2)  # exact (erf) GELU, one rounding at the store
     else:
         y = _epilogue(y, bias, rowbias, rows_per_rowbias, residual)
-    _count()
-    if out is None:
-        return y.to(torch.float16).contiguous()
-    assert out.stride(1) == 1
-    out.copy_(y.to(torch.float16))
-    return out
+    return y
 
 
 def conv3x3(x, w_packed, bias=None, rowbias=None, rows_per_rowbias=0, residual=None, out=None, n_slots=1, slot_stride=0, stride=1):
-    _f16(x, "conv3x3.x")
-    assert x.dim() == 4 and x.is_contiguous()
-    NF, H, W, C = x.shape
-    Cout = w_packed.shape[0]
-    Cin = w_packed.shape[1] // 9
-    assert w_packed.shape[1] == 9 * Cin and C <= Cin and H % stride == 0 and W % stride == 0
-    w = w_packed.double().view(Cout, 3, 3, Cin).permute(0, 3, 1, 2)[:, :C]  # [Cout][ky][kx][Cin] -> OIHW; padded channels read zeros
-    H, W = H // stride, W // stride
-    y = F.conv2d(x.double().permute(0, 3, 1, 2), w, None, stride=stride, padding=1).permute(0, 2, 3, 1).reshape(NF * H * W, Cout)
-    y = _epilogue(y, bias, rowbias, rows_per_rowbias, None)
-    M = NF * H * W
+    y = conv3x3_exact(x, w_packed, bias, rowbias, rows_per_rowbias, stride)
+    NF, H, W = x.shape[0], x.shape[1] // stride, x.shape[2] // stride
+    M, Cout = y.shape
     _count()
     if out is None:
         assert n_slots == 1
@@ -160,8 +168,29 @@ def conv3x3(x, w_packed, bias=None, rowbias=None, rows_per_rowbias=0, residual=N
     return out
 
 
+def conv3x3_exact(x, w_packed, bias=None, rowbias=None, rows_per_rowbias=0, stride=1):
+    """the float64 accumulator tile of ``conv3x3`` with bias and rowbias, [M, Cout]; each slot's residual is added to it before
+    the store rounds to fp16"""
+    _f16(x, "conv3x3.x")
+    assert x.dim() == 4 and x.is_contiguous()
+    NF, H, W, C = x.shape
+    Cout = w_packed.shape[0]
+    Cin = w_packed.shape[1] // 9
+    assert w_packed.shape[1] == 9 * Cin and C <= Cin and H % stride == 0 and W % stride == 0
+    w = w_packed.double().view(Cout, 3, 3, Cin).permute(0, 3, 1, 2)[:, :C]  # [Cout][ky][kx][Cin] -> OIHW; padded channels read zeros
+    H, W = H // stride, W // stride
+    y = F.conv2d(x.double().permute(0, 3, 1, 2), w, None, stride=stride, padding=1).permute(0, 2, 3, 1).reshape(NF * H * W, Cout)
+    return _epilogue(y, bias, rowbias, rows_per_rowbias, None)
+
+
 def upsample2x_conv3x3(x, w_phases, bias=None, out=None):
     """the four 2 x 2 phase convolutions of nearest-up x 2 + conv 3 x 3, interleaved into the [NF, 2H, 2W, Cout] image"""
+    y = upsample2x_conv3x3_exact(x, w_phases, bias)
+    _count(4)
+    return _store(out, y, y.shape)
+
+
+def upsample2x_conv3x3_exact(x, w_phases, bias=None):
     _f16(x, "upsample2x_conv3x3.x")
     NF, H, W, Cin = x.shape
     Cout = w_phases.shape[1]
@@ -172,11 +201,17 @@ def upsample2x_conv3x3(x, w_phases, bias=None, out=None):
         w = w_phases[ph].double().view(Cout, 2, 2, Cin).permute(0, 3, 1, 2)  # OIHW, tap (a, b) reads input (i + a - 1 + py, j + b - 1 + px)
         acc = F.conv2d(xp[:, :, py:py + H + 1, px:px + W + 1], w, None if bias is None else bias.double())  # [NF, Cout, H, W]
         y[:, py::2, px::2, :] = acc.permute(0, 2, 3, 1)
-        _count()
-    return _store(out, y, (NF, 2 * H, 2 * W, Cout))
+    return y
 
 
 def tconv3(x, w_packed, F_, HW, bias=None, residual=None, out=None):
+    y = tconv3_exact(x, w_packed, F_, HW, bias, residual)
+    _count()
+    return _store(out, y, (x.shape[0], x.shape[1], y.shape[1]))
+
+
+def tconv3_exact(x, w_packed, F_, HW, bias=None, residual=None):
+    """the float64 value ``tconv3`` rounds to fp16 at the store, [B * F * HW, Cout]"""
     _f16(x, "tconv3.x")
     assert x.dim() == 3 and x.is_contiguous() and x.shape[1] == F_ * HW
     B, R, Cin = x.shape
@@ -184,23 +219,52 @@ def tconv3(x, w_packed, F_, HW, bias=None, residual=None, out=None):
     w = w_packed.double().view(Cout, 3, Cin).permute(0, 2, 1)[:, :, :, None, None]  # [Cout][kt][Cin] -> [O, I, kt, 1, 1]
     x5 = x.double().view(B, F_, HW, 1, Cin).permute(0, 4, 1, 2, 3)
     y = F.conv3d(x5, w, None, padding=(1, 0, 0)).permute(0, 2, 3, 4, 1).reshape(B * R, Cout)
-    y = _epilogue(y, bias, None, 0, None if residual is None else residual.reshape(B * R, Cout))
-    _count()
-    return _store(out, y, (B, R, Cout))
+    return _epilogue(y, bias, None, 0, None if residual is None else residual.reshape(B * R, Cout))
 
 
 # ------------------------------------------------------------------------------------------------------------- attention
 def attention(q, k, v, heads, seq, batch, out, scale=0.125, n_v=1, v_branch_stride=0, o_branch_stride=0,
               frames_mode=False, HW=0, seq_kv=0, kv_batch_div=0):
+    def store(rows, o, c):
+        out[rows, :o.shape[1]] = o.to(torch.float16)
+
+    _attention(q, k, v, heads, seq, batch, out, scale, n_v, v_branch_stride, o_branch_stride, frames_mode, HW, seq_kv,
+               kv_batch_div, store)
+    _count()
+    return out
+
+
+def attention_exact(q, k, v, heads, seq, batch, out, scale=0.125, n_v=1, v_branch_stride=0, o_branch_stride=0,
+                    frames_mode=False, HW=0, seq_kv=0, kv_batch_div=0, cond=None):
+    """the float64 values ``attention`` rounds to fp16 at the store, as a float64 [out rows, heads * 64] matrix (NaN where
+    nothing is stored).  cond(p, qh, kh, vh, o) -> a tensor like o: computed from the exact softmax p [..., heads, Lq, Lk] and
+    the same operands, returned in the same layout as a second matrix (None without ``cond``)"""
+    C = heads * 64
+    ref = torch.full((out.shape[0], C), float("nan"), dtype=torch.float64)
+    cnd = torch.full_like(ref, float("nan")) if cond is not None else None
+
+    def store(rows, o, c):
+        ref[rows] = o
+        if c is not None:
+            cnd[rows] = c
+
+    _attention(q, k, v, heads, seq, batch, out, scale, n_v, v_branch_stride, o_branch_stride, frames_mode, HW, seq_kv,
+               kv_batch_div, store, cond)
+    return ref, cnd
+
+
+def _attention(q, k, v, heads, seq, batch, out, scale, n_v, v_branch_stride, o_branch_stride, frames_mode, HW, seq_kv,
+               kv_batch_div, store, cond=None):
     for name, t in (("q", q), ("k", k), ("v", v), ("o", out)):
         _f16(t, "attention." + name)
         assert t.dim() == 2 and t.stride(1) == 1
     C = heads * 64
     ldv, ldo = v.stride(0), out.stride(0)
 
-    def sdpa(qh, kh, vh):  # [..., L, heads, 64]
+    def sdpa(qh, kh, vh):  # [..., L, heads, 64] -> (o, cond(...) or None)
         p = torch.softmax(torch.einsum("...qhd,...khd->...hqk", qh.double(), kh.double()) * scale, dim=-1)
-        return torch.einsum("...hqk,...khd->...qhd", p, vh.double())
+        o = torch.einsum("...hqk,...khd->...qhd", p, vh.double())
+        return o, (None if cond is None else cond(p, qh.double(), kh.double(), vh.double(), o))
 
     branches = range(n_v)
     if not frames_mode:
@@ -213,8 +277,9 @@ def attention(q, k, v, heads, seq, batch, out, scale=0.125, n_v=1, v_branch_stri
         orows = o_branch_stride // ldo if n_v == 3 else 0
         for b in branches:
             vh = v[b * vrows:b * vrows + kvb * nk, :C].reshape(kvb, nk, heads, 64).repeat_interleave(div, dim=0)
-            o = sdpa(qh, kh, vh).reshape(batch * seq, C)
-            out[b * orows:b * orows + batch * seq, :C] = o.to(torch.float16)
+            o, c = sdpa(qh, kh, vh)
+            store(slice(b * orows, b * orows + batch * seq), o.reshape(batch * seq, C),
+                  None if c is None else c.reshape(batch * seq, C))
     else:
         assert batch % HW == 0 and (seq_kv <= 0 or seq_kv == seq) and kv_batch_div <= 1
         clips, Fr = batch // HW, seq
@@ -225,10 +290,9 @@ def attention(q, k, v, heads, seq, batch, out, scale=0.125, n_v=1, v_branch_stri
         orows = o_branch_stride // ldo if n_v == 3 else 0
         for b in branches:
             vh = to_seq(v[b * vrows:b * vrows + rows, :C])
-            o = sdpa(qh, kh, vh).permute(0, 2, 1, 3, 4).reshape(rows, C)  # back to frame-major tokens
-            out[b * orows:b * orows + rows, :C] = o.to(torch.float16)
-    _count()
-    return out
+            o, c = sdpa(qh, kh, vh)
+            back = lambda t: t.permute(0, 2, 1, 3, 4).reshape(rows, C)  # back to frame-major tokens
+            store(slice(b * orows, b * orows + rows), back(o), None if c is None else back(c))
 
 
 def temporal_attention_fused(x, wqkv, heads, F_, HW, clips, out, scale=0.125, n_v=1):
