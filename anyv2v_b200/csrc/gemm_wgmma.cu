@@ -7,10 +7,13 @@
 // channels-last activations — the A row of output pixel m for K block kb is the (tap, channel block) the block names, so the
 // 3 x 3 conv (plain, stride 2, one phase of nearest-up x 2), the temporal (3, 1, 1) conv and the two-source skip concat are
 // implicit GEMMs without an im2col buffer; out-of-image taps, ragged rows and the K tail are zero-filled by cp.async.
-// kStages = 4 stage ring (32 KB per stage), prefetch distance 2, one wgmma group in flight behind the current one:
+// kStages = 3 stage ring (32 KB per stage), prefetch distance 1, one wgmma group in flight behind the current one:
 //   top of K block kb: cp.async of block kb landed (wait_group) -> fence.proxy.async -> __syncthreads (also: every warpgroup
 //   retired wgmma kb-2)
-//   -> issue the loads of block kb + 2 into the slot of kb - 2 -> wgmma kb -> wait_group 1 (kb - 1 retired).
+//   -> issue the loads of block kb + 1 into the slot of kb - 2 -> wgmma kb -> wait_group 1 (kb - 1 retired).
+// Two CTAs per SM (2 x 97 KB of shared memory, <= 128 registers per thread): one CTA's prologue loads, K-loop gathers and
+// epilogue run while the other's wgmma keep the tensor cores busy.  A tile's K loop is short (5 blocks at K = 320), so
+// this overlap between tiles is worth more than a deeper ring inside one: with 4 stages only one CTA fits.
 // Epilogue from the accumulator registers: + bias / rowbias / residual per slot, fp16 pairs stored directly; GEGLU pairs the
 // h and gate columns (blocks of 32, interleaved by geglu_pack) which the accumulator layout puts in the same thread.
 #include "host_util.cuh"
@@ -20,7 +23,7 @@ namespace av2v {
 namespace {
 
 constexpr int BM = 128, BN = 128, BK = 64;
-constexpr int kStages = 4;
+constexpr int kStages = 3;
 constexpr int kThreads = 256;
 constexpr int kTileBytes = BM * BK * 2;  // 16 KB, A and B alike (BM == BN)
 constexpr int kSmemBytes = kStages * 2 * kTileBytes + 1024;
@@ -146,7 +149,7 @@ __device__ __forceinline__ void load_stage(const GemmP& p, const ARows& ar, int 
   }
 }
 
-__global__ void __launch_bounds__(kThreads, 1) gemm_wgmma_kernel(const __grid_constant__ GemmP p) {
+__global__ void __launch_bounds__(kThreads, 2) gemm_wgmma_kernel(const __grid_constant__ GemmP p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t s0 = smem_u32(smem);
