@@ -93,9 +93,9 @@ def fourier_filter_closed_form(x, s):
     [H//2-1 : H//2+1]^2 holds the modes {0, -1} of each axis (only {0} on a size-1 axis), so y = x + (s - 1) / (H W) * the sum
     over those modes of Re(X[mode] e^{-i angle}).  Evaluated in x's dtype (float64 in the contract)."""
     H, W = x.shape[-3], x.shape[-2]
-    th = (2 * math.pi / H) * torch.arange(H, dtype=x.dtype)[:, None].expand(H, W)
-    ph = (2 * math.pi / W) * torch.arange(W, dtype=x.dtype)[None, :].expand(H, W)
-    angles = [torch.zeros(H, W, dtype=x.dtype)]
+    th = (2 * math.pi / H) * torch.arange(H, dtype=x.dtype, device=x.device)[:, None].expand(H, W)
+    ph = (2 * math.pi / W) * torch.arange(W, dtype=x.dtype, device=x.device)[None, :].expand(H, W)
+    angles = [torch.zeros(H, W, dtype=x.dtype, device=x.device)]
     if H > 1:
         angles.append(th)
     if W > 1:

@@ -9,7 +9,9 @@ de-duplication / pruning switches can be checked for bit-identical results), and
 on top of the kernels (the channels-last UNet wiring, the PnP de-duplication, hooks, loops, latent store) run on CPU and
 be compared with the oracle.  tests/test_gpu_contracts.py runs every kernel against these functions on the GPU (guarded
 buffers, same views and strides), so the contract the CPU tests rely on is the one the kernels implement;
-tests/test_gpu_kernels.py checks them against inline fp32 formulas as well.  Nothing outside tests/ imports this file.
+tests/test_gpu_kernels.py checks them against inline fp32 formulas as well.  Every function computes on its inputs' device,
+so tests/call_audit.py evaluates the same contracts on the GPU for the calls of a full-size pass.  Nothing outside tests/
+imports this file.
 """
 from __future__ import annotations
 
@@ -114,7 +116,7 @@ def _epilogue(y, bias, rowbias, rows_per_rowbias, residual2d):
     if bias is not None:
         y = y + bias.double()
     if rowbias is not None:
-        idx = torch.arange(y.shape[0]) // rows_per_rowbias
+        idx = torch.arange(y.shape[0], device=y.device) // rows_per_rowbias
         y = y + rowbias.double()[idx]
     if residual2d is not None:
         y = y + residual2d.double()
@@ -195,7 +197,7 @@ def upsample2x_conv3x3_exact(x, w_phases, bias=None):
     NF, H, W, Cin = x.shape
     Cout = w_phases.shape[1]
     xp = F.pad(x.double().permute(0, 3, 1, 2), (1, 1, 1, 1))  # zero border: input offsets -1 .. +1
-    y = torch.zeros(NF, 2 * H, 2 * W, Cout, dtype=torch.float64)
+    y = torch.zeros(NF, 2 * H, 2 * W, Cout, dtype=torch.float64, device=x.device)
     for ph in range(4):
         py, px = ph >> 1, ph & 1
         w = w_phases[ph].double().view(Cout, 2, 2, Cin).permute(0, 3, 1, 2)  # OIHW, tap (a, b) reads input (i + a - 1 + py, j + b - 1 + px)
@@ -240,7 +242,7 @@ def attention_exact(q, k, v, heads, seq, batch, out, scale=0.125, n_v=1, v_branc
     nothing is stored).  cond(p, qh, kh, vh, o) -> a tensor like o: computed from the exact softmax p [..., heads, Lq, Lk] and
     the same operands, returned in the same layout as a second matrix (None without ``cond``)"""
     C = heads * 64
-    ref = torch.full((out.shape[0], C), float("nan"), dtype=torch.float64)
+    ref = torch.full((out.shape[0], C), float("nan"), dtype=torch.float64, device=q.device)
     cnd = torch.full_like(ref, float("nan")) if cond is not None else None
 
     def store(rows, o, c):
@@ -295,19 +297,31 @@ def _attention(q, k, v, heads, seq, batch, out, scale, n_v, v_branch_stride, o_b
             store(slice(b * orows, b * orows + rows), back(o), None if c is None else back(c))
 
 
-def temporal_attention_fused(x, wqkv, heads, F_, HW, clips, out, scale=0.125, n_v=1):
-    """Q/K/V projection (rounded to fp16, as the QKV GEMM would store them) + frames-mode attention; n_v = 3: Q, K of every
-    clip from the source clip of the same index (clips ordered [source | uncond | cond])"""
+def _tattn_operands(x, wqkv, heads, F_, HW, clips, out, scale, n_v):
+    """Q/K/V projection (rounded to fp16, as the QKV GEMM would store them) and the frames-mode ``attention`` arguments that
+    read them; n_v = 3: Q, K of every clip from the source clip of the same index (clips ordered [source | uncond | cond])"""
     _f16(x, "temporal_attention_fused.x")
     C = heads * 64
     qkv = (x.double() @ wqkv.double().t()).to(torch.float16)
-    _count(0)
     if n_v == 1:
-        return attention(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], heads, F_, clips * HW, out, scale=scale, frames_mode=True, HW=HW)
+        return (qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], heads, F_, clips * HW, out), dict(scale=scale, frames_mode=True, HW=HW)
     assert n_v == 3 and clips % 3 == 0
     src_rows = (clips // 3) * F_ * HW
-    return attention(qkv[:src_rows, :C], qkv[:src_rows, C:2 * C], qkv[:, 2 * C:], heads, F_, (clips // 3) * HW, out, scale=scale, n_v=3,
-                     v_branch_stride=src_rows * qkv.stride(0), o_branch_stride=src_rows * out.stride(0), frames_mode=True, HW=HW)
+    return ((qkv[:src_rows, :C], qkv[:src_rows, C:2 * C], qkv[:, 2 * C:], heads, F_, (clips // 3) * HW, out),
+            dict(scale=scale, n_v=3, v_branch_stride=src_rows * qkv.stride(0), o_branch_stride=src_rows * out.stride(0),
+                 frames_mode=True, HW=HW))
+
+
+def temporal_attention_fused(x, wqkv, heads, F_, HW, clips, out, scale=0.125, n_v=1):
+    """the fused projection + temporal attention: ``attention`` on the fp16-rounded projections (_tattn_operands)"""
+    args, kw = _tattn_operands(x, wqkv, heads, F_, HW, clips, out, scale, n_v)
+    return attention(*args, **kw)
+
+
+def temporal_attention_fused_exact(x, wqkv, heads, F_, HW, clips, out, scale=0.125, n_v=1, cond=None):
+    """the float64 values ``temporal_attention_fused`` rounds to fp16 at the store, as ``attention_exact`` returns them"""
+    args, kw = _tattn_operands(x, wqkv, heads, F_, HW, clips, out, scale, n_v)
+    return attention_exact(*args, cond=cond, **kw)
 
 
 CONTRACTS = dict(upsample2x_conv3x3=upsample2x_conv3x3, temporal_attention_fused=temporal_attention_fused, ddim_step=ddim_step, groupnorm=groupnorm, layernorm=layernorm, geglu_pack=geglu_pack, linear=linear,

@@ -7,7 +7,8 @@ import torch
 
 import freeu_ref
 from guarded import check_output, guarded_inout, guarded_input, guarded_output
-from parity_utils import assert_fp16_close, err_stats
+from parity_utils import err_stats
+from ulp_check import KAPPA_FREEU, assert_within_bound, cond_freeu
 
 pytestmark = pytest.mark.gpu
 dev = "cuda"
@@ -15,7 +16,7 @@ FREEU = dict(s1=0.9, s2=0.2, b1=1.5, b2=1.6)
 
 
 def _check_freeu(hidden, skip, b, s):
-    """ops.freeu on guarded CUDA views vs the contract on CPU copies: the filtered skip to fp16 tolerance, hidden[..., :C/2]
+    """ops.freeu on guarded CUDA views vs the contract on CPU copies: the filtered skip within the FreeU bound, hidden[..., :C/2]
     bit for bit against torch's fp16 `h * b` on the GPU, hidden[..., C/2:], the skip and every guard untouched"""
     from anyv2v_b200 import ops
     NF, H, W, Cs = skip.shape
@@ -34,7 +35,10 @@ def _check_freeu(hidden, skip, b, s):
     h_host = hidden.clone()
     ref = freeu_ref.freeu(h_host, skip, b, s)
     assert torch.equal(gh.view.cpu(), h_host), "hidden differs from the contract"
-    assert_fp16_close(go.view.cpu(), ref, f"freeu {tuple(skip.shape)} s={s}")
+    exact = freeu_ref.fourier_filter_closed_form(skip.double(), float(torch.tensor(s, dtype=torch.float32)))
+    assert torch.equal(ref, exact.half())
+    assert_within_bound(go.view.cpu(), exact, cond_freeu(skip, s), KAPPA_FREEU, f"freeu {tuple(skip.shape)} s={s}",
+                        shape=tuple(skip.shape))
 
 
 @pytest.mark.parametrize("shape,ch", [((48, 8, 8, 1280), 1280), ((48, 16, 16, 1280), 1280), ((48, 16, 16, 640), 1280),

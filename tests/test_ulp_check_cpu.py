@@ -9,8 +9,8 @@ import pytest
 import torch
 
 import kernel_contracts as kc
-from ulp_check import (KAPPA_GEGLU, KAPPA_GEMM, KAPPA_NORM, assert_within_bound, cond_layernorm, cond_linear, measure,
-                       ulp16)
+from ulp_check import (KAPPA_FREEU, KAPPA_GEGLU, KAPPA_GEMM, KAPPA_NORM, assert_within_bound, cond_freeu, cond_layernorm,
+                       cond_linear, measure, ulp16)
 
 f32 = np.float32
 
@@ -263,6 +263,47 @@ def test_groupnorm_unshifted_sums_fail():
 def test_groupnorm_shifted_sums_pass(ratio):
     x, gm, bt = _gn_inputs(ratio)
     _gn_check(x, gm, bt, True, f"groupnorm shifted sums, |mean| / sigma = {ratio}")
+
+
+# ------------------------------------------------------------------------------------------------------------- FreeU
+def _freeu_filter(x, s, fp16_sums):
+    """csrc/freeu.cu's filtered skip of one channels-last plane x[H, W, C]: seven plane sums of x * t over the H W pixels,
+    accumulated one pixel after the other (fp32, or fp16 with fp16_sums), twiddles t = cos / sin of th_h, ph_w, th_h + ph_w
+    rounded to fp32, then y = fp16(x + sum_j ((s - 1) / (H W) * S_j) * t_j)"""
+    H, W, C = x.shape
+    th = 2 * np.pi * np.arange(H)[:, None] / H + 0 * np.arange(W)[None, :]
+    ph = 0 * np.arange(H)[:, None] + 2 * np.pi * np.arange(W)[None, :] / W
+    t = [np.ones((H, W))] + [fn(a) for a in (th, ph, th + ph) for fn in (np.cos, np.sin)]
+    t = [tj.reshape(H * W, 1).astype(f32) for tj in t]
+    xs = x.numpy().astype(f32).reshape(H * W, C)
+    acc = np.float16 if fp16_sums else f32
+    k = f32(f32(s) - f32(1.0)) / f32(H * W)
+    corr = np.zeros((H * W, C), f32)
+    for tj in t:
+        S = np.cumsum((xs * tj).astype(acc), axis=0, dtype=acc)[-1].astype(f32)
+        corr = (corr + (k * S).astype(f32) * tj).astype(f32)
+    return torch.from_numpy((xs + corr).astype(np.float16).reshape(H, W, C))
+
+
+def _freeu_plane(seed=0, H=32, W=32, C=64):
+    """planes with a per-channel offset of 2 +- 1, so the mode-0 sums are large: 2 H W"""
+    g = torch.Generator().manual_seed(seed)
+    return (torch.randn(H, W, C, generator=g) + 2 + torch.rand(1, 1, C, generator=g) * 2 - 1).half()
+
+
+@pytest.mark.parametrize("s", [0.2, 0.9, 1.6])
+def test_freeu_fp32_plane_sums_pass(s):
+    import freeu_ref
+    x = _freeu_plane()
+    ref = freeu_ref.fourier_filter_closed_form(x.double(), float(f32(s)))
+    assert_within_bound(_freeu_filter(x, s, False), ref, cond_freeu(x, s), KAPPA_FREEU, f"freeu fp32 plane sums, s = {s}")
+
+
+def test_freeu_fp16_plane_sums_fail():
+    import freeu_ref
+    x = _freeu_plane()
+    ref = freeu_ref.fourier_filter_closed_form(x.double(), float(f32(0.2)))
+    _fails(_freeu_filter(x, 0.2, True), ref, cond_freeu(x, 0.2), KAPPA_FREEU)
 
 
 def test_measure_reports_margin():

@@ -31,6 +31,10 @@ KAPPA_NORM = 2.0 ** -20
 # attention: P is rounded to fp16 before the PV product by design (the wgmma A fragment is fp16), a relative error of
 # 2^-11 per weight of |V|: 2^-10 covers it and the fp32 exponentials.
 KAPPA_ATTN = 2.0 ** -10
+# FreeU's filtered skip, y = x + (s - 1) / (H W) * sum_j S_j t_j (tests/freeu_ref.py): each of the seven plane sums S_j adds
+# H W fp32 products x * t with |t| <= 1, so it keeps (H W) 2^-24 of sum |x|; the twiddles t carry <= 3 * 2^-24 in both passes,
+# and (s - 1) / (H W) cancels the H W: |err| <= 2^-24 (|x| + 7 |s - 1| sum |x| (1 + 3 + 3 + 1)) <= 2^-21 * cond_freeu.
+KAPPA_FREEU = 2.0 ** -20
 
 FP16_MAX_FINITE_EDGE = 65520.0  # values at or above this magnitude round to inf in fp16
 
@@ -43,9 +47,9 @@ def ulp16(ref: torch.Tensor) -> torch.Tensor:
 
 def measure(got16: torch.Tensor, ref64: torch.Tensor, cond64: torch.Tensor, kappa: float) -> dict:
     """worst element statistics: error in ulps, error over the bound (negative = margin), fraction over the bound"""
-    got = torch.as_tensor(got16).detach().to("cpu", torch.float64).reshape(-1)
-    ref64 = torch.as_tensor(ref64).detach().to("cpu", torch.float64)
-    cond = torch.broadcast_to(torch.as_tensor(cond64, dtype=torch.float64).cpu(), ref64.shape).reshape(-1)
+    ref64 = torch.as_tensor(ref64).detach().to(torch.float64)  # evaluated on ref64's device
+    got = torch.as_tensor(got16).detach().to(ref64.device, torch.float64).reshape(-1)
+    cond = torch.broadcast_to(torch.as_tensor(cond64, dtype=torch.float64).to(ref64.device), ref64.shape).reshape(-1)
     ref = ref64.reshape(-1)
     assert got.shape == ref.shape == cond.shape, (got.shape, ref.shape, cond.shape)
     assert torch.isfinite(ref).all() and torch.isfinite(cond).all(), "reference or condition scale not finite"
@@ -81,7 +85,8 @@ def assert_within_bound(got16, ref64, cond64, kappa: float, what: str, shape=Non
 
 # ------------------------------------------------------------------------------------------------------------- cond per op
 def _d(t):
-    return None if t is None else torch.as_tensor(t).detach().to("cpu", torch.float64)
+    """float64 on the tensor's own device"""
+    return None if t is None else torch.as_tensor(t).detach().to(torch.float64)
 
 
 def cond_linear(a, w, bias=None, rowbias=None, rows_per_rowbias=0, residual=None, a2=None):
@@ -91,7 +96,7 @@ def cond_linear(a, w, bias=None, rowbias=None, rows_per_rowbias=0, residual=None
     if bias is not None:
         c = c + _d(bias).abs()
     if rowbias is not None:
-        c = c + _d(rowbias).abs()[torch.arange(c.shape[0]) // rows_per_rowbias]
+        c = c + _d(rowbias).abs()[torch.arange(c.shape[0], device=c.device) // rows_per_rowbias]
     if residual is not None:
         c = c + _d(residual).abs().reshape(c.shape)
     return c
@@ -169,3 +174,12 @@ def cond_attention(scale, rounded_operands=False):
             return 2 * pv + (2.0 ** -8 + 2.0) * dev
         return pv + 2.0 ** -8 * dev
     return cond
+
+
+def cond_freeu(skip, s):
+    """|x| + 7 |s - 1| sum_plane |x| per element of channels-last planes skip[..., H, W, C]: the operand of the final add and
+    the magnitudes the seven plane sums add, carried through (s - 1) / (H W) (H W cancels against fp32 accumulation over H W
+    terms, see KAPPA_FREEU); s is the fp32 value the kernel receives"""
+    x = _d(skip).abs()
+    s32 = float(torch.tensor(s, dtype=torch.float32))
+    return x + 7.0 * abs(s32 - 1.0) * x.sum(dim=(-3, -2), keepdim=True)
