@@ -63,16 +63,19 @@ def invert_loop(unet, latents, prompt_embeds, image_latents, image_embeddings, f
 @torch.no_grad()
 def pnp_edit_loop(pipe, register_time, inv_latents: dict, latents, prompt_embeds_all, image_latents_all,
                   image_embeddings_all, fps_all, n_steps: int, guidance: float, t_idx: int = 0,
-                  scheduler: DDIMScheduler | None = None):
-    """pipe: object with .unet whose hooks were registered by init_pnp. Returns final latents [1,4,F,h,w]."""
+                  scheduler: DDIMScheduler | None = None, callback=None):
+    """pipe: object with .unet whose hooks were registered by init_pnp. Returns final latents [1,4,F,h,w].
+    ``callback(i, t, latents)`` (optional) sees the latents after every step, as the pipeline's callback does."""
     sched = scheduler or DDIMScheduler()
     sched.set_timesteps(n_steps)
-    for t in sched.timesteps[t_idx:]:
+    for i, t in enumerate(sched.timesteps[t_idx:]):
         x_in = torch.cat([inv_latents[int(t)], latents, latents])
         register_time(pipe, int(t))
         v = pipe.unet(x_in, t, fps_all, image_latents_all, image_embeddings_all, prompt_embeds_all)[0]
         _, v_neg, v_edit = v.chunk(3)
         latents, _ = sched.step(cfg_combine(v_neg, v_edit, guidance), int(t), latents)
+        if callback is not None:
+            callback(i, int(t), latents)
     return latents
 
 

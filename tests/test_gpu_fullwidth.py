@@ -30,13 +30,14 @@ def _config():
     return CONFIG_OVERRIDE or unet_ref.I2VGEN_XL_CONFIG
 
 
-def build_models(device):
+def build_models(device, config=None):
+    """config: None = this module's _config() (other modules pass their own override)"""
     from anyv2v_b200.unet_i2vgen_xl import I2VGEN_XL_CONFIG, I2VGenXLUNet
     from oracle import unet_ref
     assert I2VGEN_XL_CONFIG == unet_ref.I2VGEN_XL_CONFIG
-    cfg = _config()
+    cfg = config or _config()
     ref32 = unet_ref.seeded_unet(cfg, seed=8888, dtype=torch.float32, device="cpu")
-    if CONFIG_OVERRIDE is None:
+    if cfg == unet_ref.I2VGEN_XL_CONFIG:
         n_params = sum(p.numel() for p in ref32.parameters())
         assert n_params == 1_420_469_224, n_params
     with torch.device("meta"):
