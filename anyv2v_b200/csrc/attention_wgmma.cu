@@ -6,7 +6,9 @@
 // (running max / sum per row, base-2 exponentials; a quarter of them on the FMA pipe, ex2_poly), converts P to fp16 in
 // registers — the accumulator layout of S is the A-fragment layout of the next wgmma — and accumulates O += P V with V read
 // MN-major ([keys][64], 64 contiguous) from shared memory.  With n_v = 3 (injected step) ONE P feeds the V of all three
-// branches.  K / V tiles are double-buffered with cp.async.
+// branches.  K / V tiles are double-buffered with cp.async.  Rows-mode calls with 512 keys or more run attn_rows_kernel
+// instead: the same per-row algorithm, warp-specialized (TMA producer warp, mbarrier stage ring, two consumer warpgroups taking
+// turns at the tensor cores).
 //
 // Query slots map to token rows by mode:
 //   rows   : slot i of q tile qt -> token qt * 128 + i of sequence b; keys = the b / kv_batch_div-th key sequence.
@@ -245,6 +247,237 @@ __global__ void __launch_bounds__(kThreads) attn_kernel(const __grid_constant__ 
 template <int NV>
 constexpr int attn_smem() { return 2 * kTile + 2 * (1 + NV) * kTile + 1024; }
 
+// --------------------------------------------------------------------------------------------------- rows mode, pipelined
+// attn_rows_kernel: the rows-mode path of av2v_attn_pnp_f16, warp-specialized.  384 threads: warpgroup 0 is the producer (one
+// thread issues TMA loads; registers lowered to 40), warpgroups 1 and 2 are the consumers (64 query rows each; raised to 232).
+// Q (128 rows) is loaded once; K and the NV V tiles of each key tile go through a ring of kRowsStages stages, each with a
+// full mbarrier (producer arrive + TMA bytes) and an empty mbarrier (one arrive per consumer warp once the wgmma reading the
+// stage retired).  The tensor maps zero-fill keys past seq_kv and query rows past seq, so 0 * NaN never reaches PV.
+// The consumers alternate their MMA issue through named barriers 1 and 2 (ping-pong): per turn a warpgroup issues PV of tile j
+// and S = Q K^T of tile j + 1 as one wgmma group, hands the turn over, waits for the group, releases stage j and runs the
+// softmax of tile j + 1 under the other warpgroup's MMAs.
+// Key tile: 128 keys at NV = 1 (S m64n128, half the rescale work of 64); 64 at NV = 3, where O alone holds 96 registers and
+// S + P of 128 keys would not fit the 168 a thread of a 384-thread CTA is compiled for.
+// Per-row algorithm as attn_tile: running max over raw scores, x = s * scale_log2 - ref in one FMA, a quarter of the
+// exponentials (key columns 24-31 of every 32) on the FMA pipe, fp16 P as the register A operand of PV, one division by l at
+// the store.
+template <int NV>
+__host__ __device__ constexpr int rows_keys() { return NV == 1 ? 128 : 64; }
+constexpr int kRowsStages = 6;  // 6 x (K + NV V tiles): 192 KB at either NV, 1 CTA per SM
+template <int NV>
+constexpr int rows_smem() { return 2 * kTile + kRowsStages * (1 + NV) * rows_keys<NV>() * 128 + 1024; }
+constexpr int kRowsThreads = 384;
+// Rows-mode calls with fewer keys stay on attn_kernel: with one CTA per SM, the prologue (Q and the first stage in flight) and
+// the store are not hidden behind another CTA, and a key loop of 4 tiles or fewer does not pay for them (tools/attn_bench.py:
+// 64- and 256-token self-attention and 145-key cross-attention are no faster, 1024- and 4096-token self-attention 2x faster).
+constexpr int kRowsMinKeys = 512;
+
+struct AttnRowsP {
+  CUtensorMap tq, tk, tv;  // 4-D (column, token, sequence, V branch) fp16 maps, boxes 64 x 128 (Q) / 64 x key tile (K, V)
+  __half* o;
+  int ldo, heads, seq, seq_kv, kv_div, q_tiles;
+  long long o_branch_stride;
+  float scale_log2;
+};
+
+// softmax of one score tile (N = 2 * key tile / 4 registers) in place -> fp16 P fragments; rescales O and l by the raised
+// running max.  kMask: keys at columns >= lim are past seq_kv.
+template <int NV, int N, bool kMask>
+__device__ __forceinline__ void rows_softmax(float (&s)[N], uint32_t (&pa)[N / 8][4], float (&o)[NV][32], float (&m)[2],
+                                             float (&l)[2], float scale_log2, int lim) {
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int i = 0; i < N; ++i) {
+    if (kMask && acc_col(i) >= lim) s[i] = -INFINITY;
+    mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
+  }
+  float corr[2], nref[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+    mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+    const float mn = fmaxf(m[h], mx[h] * scale_log2);
+    const float ref = mn == -INFINITY ? 0.f : mn;  // a row with every key masked so far keeps p = 0
+    corr[h] = ex2_approx(m[h] - ref);
+    nref[h] = -ref;
+    m[h] = mn;
+    l[h] *= corr[h];
+  }
+#pragma unroll
+  for (int b = 0; b < NV; ++b)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[b][i] *= corr[(i >> 1) & 1];
+#pragma unroll
+  for (int i = 0; i < N; ++i) {
+    const float x = fmaf(s[i], scale_log2, nref[(i >> 1) & 1]);
+    s[i] = ((i >> 2) & 3) == 3 ? ex2_poly(x) : ex2_approx(x);
+    l[(i >> 1) & 1] += s[i];
+  }
+#pragma unroll
+  for (int kk = 0; kk < N / 8; ++kk)
+#pragma unroll
+    for (int r = 0; r < 4; ++r) pa[kk][r] = pack_half2(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
+}
+
+template <int NV>
+__global__ void __launch_bounds__(kRowsThreads, 1) attn_rows_kernel(const __grid_constant__ AttnRowsP p) {
+  constexpr int S = kRowsStages, KT = rows_keys<NV>(), N = KT / 2;
+  constexpr uint32_t kKV = KT * 128;  // bytes of one K or V tile
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t full[S], empty[S], qbar;
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const uint32_t sQ = smem_u32(smem);
+  auto sK = [&](int s) { return sQ + 2 * kTile + s * (1 + NV) * kKV; };
+  auto sV = [&](int s, int b) { return sK(s) + (1 + b) * kKV; };
+
+  int item = blockIdx.x;
+  const int qt = item % p.q_tiles;
+  item /= p.q_tiles;
+  const int h = item % p.heads;
+  const int b = item / p.heads;
+  const int n_kv = (p.seq_kv + KT - 1) / KT;
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 8);  // lane 0 of each consumer warp
+    }
+    mbar_init(&qbar, 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  const int role = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 7), 0);  // warp-uniform for ptxas
+  if (role == 0) {  // ---- producer
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      mbar_arrive_expect_tx(&qbar, 2 * kTile);
+      tma_load_4d(sQ, &p.tq, &qbar, h * HD, qt * 128, b, 0);
+      const int kvb = b / p.kv_div;
+      for (int j = 0; j < n_kv; ++j) {
+        const int s = j % S;
+        if (j >= S) mbar_wait<false>(&empty[s], ((j / S) - 1) & 1);  // both consumers released tile j - S
+        mbar_arrive_expect_tx(&full[s], (1 + NV) * kKV);
+        tma_load_4d(sK(s), &p.tk, &full[s], h * HD, j * KT, kvb, 0);
+#pragma unroll
+        for (int vb = 0; vb < NV; ++vb) tma_load_4d(sV(s, vb), &p.tv, &full[s], h * HD, j * KT, kvb, vb);
+      }
+    }
+    return;
+  }
+
+  // ---- consumers
+  setmaxnreg_inc<232>();
+  const int wg = role - 1;
+  const uint32_t q_wg = sQ + wg * kTile;
+  float o[NV][32];
+#pragma unroll
+  for (int vb = 0; vb < NV; ++vb)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[vb][i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float s[N];
+  uint32_t pa[N / 8][4];
+  auto issue_s = [&](int j) {
+#pragma unroll
+    for (int k = 0; k < HD / 16; ++k) {
+      if constexpr (KT == 128) wgmma_m64n128_ss(s, sw128_desc(q_wg + k * 32), sw128_desc(sK(j % S) + k * 32), k > 0);
+      else wgmma_m64n64_ss<0>(s, sw128_desc(q_wg + k * 32), sw128_desc(sK(j % S) + k * 32), k > 0);
+    }
+  };
+  auto issue_pv = [&](int j) {
+#pragma unroll
+    for (int vb = 0; vb < NV; ++vb)
+#pragma unroll
+      for (int kk = 0; kk < KT / 16; ++kk) wgmma_m64n64_rs<1>(o[vb], pa[kk], sw128_desc(sV(j % S, vb) + kk * 2048), 1);
+  };
+  auto softmax = [&](int j) {
+    const int lim = p.seq_kv - j * KT;
+    if (lim >= KT) rows_softmax<NV, N, false>(s, pa, o, m, l, p.scale_log2, lim);
+    else rows_softmax<NV, N, true>(s, pa, o, m, l, p.scale_log2, lim);
+  };
+  // turn taking: warpgroup w waits on barrier 1 + w and hands over with an arrive on the other.  Every turn of one warpgroup
+  // is matched by one turn of the other, so warpgroup 1's arrive ahead of its first turn stands in for one after its last.
+  auto my_turn = [&] { if (wg == 0) named_bar_sync(1, 256); else named_bar_sync(2, 256); };
+  auto hand_over = [&] { if (wg == 0) named_bar_arrive(2, 256); else named_bar_arrive(1, 256); };
+  auto release = [&](int j) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[j % S]);
+  };
+
+  if (wg == 1) named_bar_arrive(1, 256);  // warpgroup 0 takes the first turn
+  mbar_wait<false>(&qbar, 0);
+  mbar_wait<false>(&full[0], 0);
+  my_turn();
+  wgmma_fence();
+  issue_s(0);
+  wgmma_commit();
+  hand_over();
+  wgmma_wait<0>();
+  reg_fence(s);
+  softmax(0);
+  for (int j = 0; j + 1 < n_kv; ++j) {
+    mbar_wait<false>(&full[(j + 1) % S], ((j + 1) / S) & 1);
+    my_turn();
+    wgmma_fence();
+    issue_pv(j);
+    issue_s(j + 1);
+    wgmma_commit();
+    hand_over();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int vb = 0; vb < NV; ++vb) reg_fence(o[vb]);
+    reg_fence(s);
+    release(j);
+    softmax(j + 1);
+  }
+  my_turn();
+  wgmma_fence();
+  issue_pv(n_kv - 1);
+  wgmma_commit();
+  if (wg == 0) named_bar_arrive(2, 256);
+  wgmma_wait<0>();
+#pragma unroll
+  for (int vb = 0; vb < NV; ++vb) reg_fence(o[vb]);
+  release(n_kv - 1);
+
+  __half* ob[NV];
+#pragma unroll
+  for (int vb = 0; vb < NV; ++vb) ob[vb] = p.o + vb * p.o_branch_stride + h * HD;
+  store_o<NV>(o, l, ob, wg, [&](int i) -> long long {
+    const int t = qt * 128 + i;
+    return t < p.seq ? (static_cast<long long>(b) * p.seq + t) * p.ldo : -1;
+  });
+}
+
+// 4-D fp16 tensor map over [branches][sequences][tokens][cols] (row stride ld elements, branch stride in elements): a box of
+// 64 columns x box_rows tokens, 128-byte swizzle (the sw128 tile layout), zeros outside the tensor
+int encode_rows_map(CUtensorMap* map, const void* base, int cols, int tokens, int seqs, int branches, int ld,
+                    long long branch_stride, int box_rows) {
+  using Encode = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                              const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                              CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+  static Encode encode = nullptr;
+  if (encode == nullptr) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    AV2V_CHECK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
+    AV2V_REQUIRE(q == cudaDriverEntryPointSuccess && fn != nullptr, AV2V_ECUDA, "attn: cuTensorMapEncodeTiled not available");
+    encode = reinterpret_cast<Encode>(fn);
+  }
+  const cuuint64_t seq_bytes = static_cast<cuuint64_t>(tokens) * ld * 2;
+  const cuuint64_t dims[4] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(tokens), static_cast<cuuint64_t>(seqs),
+                              static_cast<cuuint64_t>(branches)};
+  const cuuint64_t strides[3] = {static_cast<cuuint64_t>(ld) * 2, seq_bytes,
+                                 branches > 1 ? static_cast<cuuint64_t>(branch_stride) * 2 : seq_bytes * seqs};
+  const cuuint32_t box[4] = {HD, static_cast<cuuint32_t>(box_rows), 1, 1}, estr[4] = {1, 1, 1, 1};
+  const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  AV2V_REQUIRE(r == CUDA_SUCCESS, AV2V_ECUDA, "attn: cuTensorMapEncodeTiled failed (%d)", static_cast<int>(r));
+  return AV2V_OK;
+}
+
 // --------------------------------------------------------------------------------------------------- av2v_tattn_fused_f16
 struct TAttnP {
   const __half* x;
@@ -456,9 +689,29 @@ extern "C" int av2v_attn_pnp_f16(const av2v_attn_args* a, av2v_stream_t stream_)
   if (!attr_set) {
     AV2V_CHECK_CUDA(cudaFuncSetAttribute(attn_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn_smem<1>()));
     AV2V_CHECK_CUDA(cudaFuncSetAttribute(attn_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn_smem<3>()));
+    AV2V_CHECK_CUDA(cudaFuncSetAttribute(attn_rows_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, rows_smem<1>()));
+    AV2V_CHECK_CUDA(cudaFuncSetAttribute(attn_rows_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, rows_smem<3>()));
     attr_set = true;
   }
-  if (a->n_v == 3) attn_kernel<3><<<static_cast<unsigned>(items), kThreads, attn_smem<3>(), stream>>>(p);
+  if (a->seq_mode == AV2V_SEQ_ROWS && p.seq_kv >= kRowsMinKeys) {
+    AttnRowsP r{};
+    const int C = a->heads * HD, kv_seqs = a->batch / p.kv_div;
+    const int kt = a->n_v == 3 ? rows_keys<3>() : rows_keys<1>();
+    if (int e = encode_rows_map(&r.tq, a->q, C, a->seq, a->batch, 1, a->ldq, 0, 128)) return e;
+    if (int e = encode_rows_map(&r.tk, a->k, C, p.seq_kv, kv_seqs, 1, a->ldk, 0, kt)) return e;
+    if (int e = encode_rows_map(&r.tv, a->v, C, p.seq_kv, kv_seqs, a->n_v, a->ldv, p.v_branch_stride, kt)) return e;
+    r.o = p.o;
+    r.ldo = a->ldo;
+    r.heads = a->heads;
+    r.seq = a->seq;
+    r.seq_kv = p.seq_kv;
+    r.kv_div = p.kv_div;
+    r.q_tiles = p.q_tiles;
+    r.o_branch_stride = p.o_branch_stride;
+    r.scale_log2 = p.scale_log2;
+    if (a->n_v == 3) attn_rows_kernel<3><<<static_cast<unsigned>(items), kRowsThreads, rows_smem<3>(), stream>>>(r);
+    else attn_rows_kernel<1><<<static_cast<unsigned>(items), kRowsThreads, rows_smem<1>(), stream>>>(r);
+  } else if (a->n_v == 3) attn_kernel<3><<<static_cast<unsigned>(items), kThreads, attn_smem<3>(), stream>>>(p);
   else attn_kernel<1><<<static_cast<unsigned>(items), kThreads, attn_smem<1>(), stream>>>(p);
   AV2V_CHECK_CUDA(cudaGetLastError());
   return AV2V_OK;

@@ -47,17 +47,40 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 #ifndef AV2V_WAIT_TIMEOUT_CYCLES
 #define AV2V_WAIT_TIMEOUT_CYCLES (4000000000ll)
 #endif
+// kReport = false traps without the printf: a function call there would make ptxas serialize the wgmma of the caller.
+template <bool kReport = true>
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
     if (clock64() - t0 > AV2V_WAIT_TIMEOUT_CYCLES) {
-      printf("av2v: mbarrier wait timeout (block %d,%d thread %d bar %u parity %u)\n", blockIdx.x, blockIdx.y,
-             threadIdx.x, smem_u32(bar), parity);
+      if (kReport)
+        printf("av2v: mbarrier wait timeout (block %d,%d thread %d bar %u parity %u)\n", blockIdx.x, blockIdx.y,
+               threadIdx.x, smem_u32(bar), parity);
       __trap();
     }
   }
 }
+
+// ------------------------------------------------------------------ TMA tile load, named barriers, register reallocation
+// box of a 4-D tensor map at coordinates (c0 innermost .. c3) -> shared memory; completes `bytes` on the mbarrier (elements
+// outside the tensor arrive as zeros and still count)
+__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(smem_u32(bar))
+      : "memory");
+}
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // ------------------------------------------------------------------ cp.async (16-byte, L2-only; zero-fill when !valid)
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {

@@ -18,8 +18,10 @@ def _ex2(a: torch.Tensor, poly_mask: torch.Tensor) -> torch.Tensor:
     return torch.where(poly_mask, p, exact)
 
 
-def attention_rows(q, k, v, scale=0.125, poly=0):
-    """q [T,64], k/v [L,64] fp16 -> [T,64] fp16, one head"""
+def attention_rows(q, k, v, scale=0.125, poly=0, tk=TK, fused=False):
+    """q [T,64], k/v [L,64] fp16 -> [T,64] fp16, one head.  tk: keys per tile (attn_tile: 64; attn_rows_kernel: 128 at
+    n_v = 1, 64 at n_v = 3).  fused (attn_rows_kernel): the running max is taken over raw scores and scaled once per row,
+    and the exponent is s * scale_log2 - max in one fused multiply-add (one rounding, emulated in float64)"""
     T, L = q.shape[0], k.shape[0]
     sc = np.float32(scale * 1.4426950408889634)
     qf, kf, vf = q.float(), k.float(), v.float()
@@ -28,27 +30,30 @@ def attention_rows(q, k, v, scale=0.125, poly=0):
     o = torch.zeros(T, 64)
     # column block j = col // 8 of a tile (accumulator registers 4j .. 4j + 3 of attn_tile) goes to the polynomial when
     # (j & 3) == 3 (25 %, the kernel) / (j & 1) == 1 (50 %)
-    j8 = torch.arange(TK) // 8
-    pm = ((j8 & 3) == 3) if poly == 1 else ((j8 & 1) == 1) if poly == 2 else torch.zeros(TK, dtype=torch.bool)
-    for j in range((L + TK - 1) // TK):
-        kt, vt = kf[j * TK:(j + 1) * TK], vf[j * TK:(j + 1) * TK]
+    j8 = torch.arange(tk) // 8
+    pm = ((j8 & 3) == 3) if poly == 1 else ((j8 & 1) == 1) if poly == 2 else torch.zeros(tk, dtype=torch.bool)
+    for j in range((L + tk - 1) // tk):
+        kt, vt = kf[j * tk:(j + 1) * tk], vf[j * tk:(j + 1) * tk]
         n = kt.shape[0]
-        s = torch.full((T, TK), float("-inf"))
+        s = torch.full((T, tk), float("-inf"))
         s[:, :n] = qf @ kt.T                     # fp32 accumulate of fp16 products (tensor core)
         rmax = s.max(dim=1).values * sc
         m_new = torch.maximum(m, rmax)
         f = torch.exp2(m - m_new)  # 0 on the first tile (m = -inf)
         o, l = o * f[:, None], l * f
         m = m_new
-        a = s * sc - m[:, None]
-        p = _ex2(a.float(), pm[None, :].expand(T, TK))
+        if fused:
+            a = (s.double() * float(sc) - m.double()[:, None]).float()
+        else:
+            a = s * sc - m[:, None]
+        p = _ex2(a.float(), pm[None, :].expand(T, tk))
         l = l + p.sum(dim=1)
         p16 = p.half().float()
         o = o + p16[:, :n] @ vt
     return (o / l[:, None]).half()
 
 
-def check(T=192, L=880, mag=2.0, poly=2, seed=0, rising=False):
+def check(T=192, L=880, mag=2.0, poly=2, seed=0, rising=False, tk=TK, fused=False):
     g = torch.Generator().manual_seed(seed)
     q = (torch.randn(T, 64, generator=g) * mag).half()
     k = torch.randn(L, 64, generator=g) * mag
@@ -56,7 +61,7 @@ def check(T=192, L=880, mag=2.0, poly=2, seed=0, rising=False):
         k = k * torch.linspace(0.2, 6.0, L)[:, None]
     k = k.half()
     v = torch.randn(L, 64, generator=g).half()
-    got = attention_rows(q, k, v, poly=poly).float()
+    got = attention_rows(q, k, v, poly=poly, tk=tk, fused=fused).float()
     ref = torch.softmax(q.double() @ k.double().T * 0.125, dim=-1) @ v.double()
     err = (got.double() - ref).abs()
     tol = 2e-3 * ref.abs().max() + 1e-3 * ref.abs()

@@ -176,3 +176,85 @@ def check_epilogue(geglu_pack, N_geglu=(128, 256, 2560)):
             want = {(n * 2 * H + y) * (2 * W) + x for n in range(NF) for y in range(py, 2 * H, 2) for x in range(px, 2 * W, 2)}
             assert rows == want
     return True
+
+
+# ---------------------------------------------------------------------------------------------------------- rows attention ring
+def rows_ring_constants():
+    """(stages, empty-barrier arrivals) of attn_rows_kernel's K / V ring, as written in attention_wgmma.cu; also checks that the
+    producer and consumer waits use the parities the model assumes"""
+    s = _src("attention_wgmma.cu")
+    stages = int(re.search(r"constexpr int kRowsStages = (\d+);", s).group(1))
+    arrivals = int(re.search(r"mbar_init\(&empty\[s\], (\d+)\);", s).group(1))
+    assert "mbar_wait<false>(&empty[s], ((j / S) - 1) & 1)" in s
+    assert "mbar_wait<false>(&full[(j + 1) % S], ((j + 1) / S) & 1)" in s and "mbar_wait<false>(&full[0], 0)" in s
+    return stages, arrivals
+
+
+class _MBar:
+    """an mbarrier as the list of its phase-completion times; a parity wait succeeds once the number of completed phases has
+    the other parity (mbarrier.try_wait.parity P: the phase of parity P has completed)"""
+    def __init__(self, count):
+        self.count, self.pending, self.done = count, [], []
+
+    def arrive(self, t, n=1):
+        self.pending += [t] * n
+        if len(self.pending) >= self.count:
+            self.done.append(max(self.pending[:self.count]))
+            self.pending = self.pending[self.count:]
+
+    def wait(self, parity, t):
+        for c in [t] + sorted(x for x in self.done if x > t):
+            if sum(1 for x in self.done if x <= c) & 1 != parity:
+                return c
+        raise AssertionError(f"wait on parity {parity} never succeeds (deadlock)")
+
+
+def simulate_rows_ring(rng: random.Random, n: int, stages: int, arrivals: int = 8, release: bool = True,
+                       wrong_parity: str = "", pingpong: bool = True):
+    """attn_rows_kernel's schedule.  Producer: per tile j, wait empty[j % S] with parity ((j / S) - 1) & 1 (j >= S), arrive +
+    TMA into stage j % S (full completes when the bytes land).  Consumers w = 0, 1 (4 warps each): turn 0 issues S(0); turn
+    k = 1 .. n issues PV(k - 1) and S(k) (k < n) after waiting full[k % S] with parity (k / S) & 1; turns alternate through the
+    named barriers (w = 0 first); after the wgmma group retired, each warp arrives on empty[(k - 1) % S].  Asserts: no tile is
+    read before it landed, no stage is refilled before both consumers released it, the MMA turns alternate 0, 1, 0, 1, ...
+    Negative controls: release=False (consumer 1 never releases), wrong_parity="consumer" / "producer", pingpong=False."""
+    full = [_MBar(1) for _ in range(stages)]
+    empty = [_MBar(arrivals) for _ in range(stages)]
+    land, released, turns = {}, {}, []
+    t_prod = 0.0
+    t_wg = [rng.uniform(0, 5), rng.uniform(0, 5)]
+    handed = [0.0, None]  # handed[w]: when the other warpgroup last handed the turn to w (w = 0 starts with it)
+
+    def produce(j):
+        nonlocal t_prod
+        s = j % stages
+        if j >= stages:
+            par = ((j // stages) - 1) & 1
+            t_prod = empty[s].wait(par ^ (wrong_parity == "producer"), t_prod)
+            for w in range(2):
+                assert released[(j - stages, w)] <= t_prod, f"stage {s} refilled with tile {j} while tile {j - stages} is read"
+        t_prod += rng.uniform(0.1, 2)
+        land[j] = t_prod + rng.uniform(5, 60)
+        full[s].arrive(land[j])
+
+    for k in range(n + 1):
+        if k < n:
+            produce(k)
+        for w in range(2):
+            t = t_wg[w]
+            if k < n:
+                t = full[k % stages].wait(((k // stages) & 1) ^ (wrong_parity == "consumer"), t)
+            if pingpong:
+                assert handed[w] is not None
+                t = max(t, handed[w])
+            for tile in ([k] if k < n else []) + ([k - 1] if k > 0 else []):
+                assert land[tile] <= t, f"warpgroup {w} reads tile {tile} before it landed"
+            turns.append((t, w))
+            handed[1 - w] = t + rng.uniform(0.1, 1)
+            retire = t + rng.uniform(5, 40)
+            if k > 0 and (release or w == 0):
+                released[(k - 1, w)] = retire
+                empty[(k - 1) % stages].arrive(retire, arrivals // 2)
+            t_wg[w] = retire + rng.uniform(1, 30)  # softmax of tile k
+    order = [w for _, w in sorted(turns, key=lambda x: x[0])]
+    assert order == [0, 1] * (n + 1), "MMA turns of the two consumers do not alternate"
+    return True
