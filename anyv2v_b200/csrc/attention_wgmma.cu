@@ -12,9 +12,12 @@
 //
 // Query slots map to token rows by mode:
 //   rows   : slot i of q tile qt -> token qt * 128 + i of sequence b; keys = the b / kv_batch_div-th key sequence.
-//   frames : tokens are frame-major [clips][F][HW][*].  F <= 128 (F | 128): a CTA packs 128 / F pixels of a clip, slot i ->
-//            (pixel i / F, frame i % F), and the keys are the same 128 slots masked to the slot's own pixel.  F % 128 == 0:
-//            one pixel, slot i -> frame ft * 128 + i, keys = all F frames of the pixel.
+//   frames : tokens are frame-major [clips][F][HW][*].  F <= 128: a CTA packs ppt = floor(128 / F) pixels of a clip, slot
+//            i < ppt * F -> (pixel i / F, frame i % F), and the keys are the same 128 slots masked to the slot's own pixel.
+//            Slots ppt * F .. 127 (the tail, empty when F | 128) hold no pixel: they load as zeros, and since slot / F >= ppt
+//            for them they are never a key of a held slot, and they are never stored.  F > 128: one pixel per CTA, slot i ->
+//            frame ft * 128 + i (f_tiles = ceil(F / 128) tiles), keys = all F frames of the pixel; frames >= F are neither
+//            loaded as queries nor stored, and as keys they are zero-filled and masked.
 #include "host_util.cuh"
 #include "ptx.cuh"
 
@@ -162,8 +165,10 @@ __global__ void __launch_bounds__(kThreads) attn_kernel(const __grid_constant__ 
     item /= p.heads;
     pix0 = item % p.HW;
     clip = item / p.HW;
-    n_kv = p.F / 64;
+    n_kv = (p.F + 63) / 64;
   }
+  // packed: slot i holds pixel pix0 + i / F when that is below pix_end; tail slots (i / F >= ppt) and pixels past HW hold none
+  const int pix_end = min(pix0 + p.ppt, p.HW);
   const long long clip_row = static_cast<long long>(clip) * p.F * p.HW;
   auto qrow = [&](int i) -> long long {
     if (p.seq_mode == AV2V_SEQ_ROWS) {
@@ -172,18 +177,19 @@ __global__ void __launch_bounds__(kThreads) attn_kernel(const __grid_constant__ 
     }
     if (packed) {
       const int pix = pix0 + i / p.F;
-      return pix < p.HW ? clip_row + static_cast<long long>(i % p.F) * p.HW + pix : -1;
+      return pix < pix_end ? clip_row + static_cast<long long>(i % p.F) * p.HW + pix : -1;
     }
-    return clip_row + static_cast<long long>(qt * 128 + i) * p.HW + pix0;
+    const int f = qt * 128 + i;
+    return f < p.F ? clip_row + static_cast<long long>(f) * p.HW + pix0 : -1;
   };
   auto krow = [&](int u) -> long long {  // key u of the key sequence(s)
     if (p.seq_mode == AV2V_SEQ_ROWS)
       return u < p.seq_kv ? static_cast<long long>(b / p.kv_div) * p.seq_kv + u : -1;
     if (packed) {
       const int pix = pix0 + u / p.F;
-      return pix < p.HW ? clip_row + static_cast<long long>(u % p.F) * p.HW + pix : -1;
+      return pix < pix_end ? clip_row + static_cast<long long>(u % p.F) * p.HW + pix : -1;
     }
-    return clip_row + static_cast<long long>(u) * p.HW + pix0;
+    return u < p.F ? clip_row + static_cast<long long>(u) * p.HW + pix0 : -1;
   };
   const int hc = h * HD;
   auto load_kv = [&](int kt, int buf) {
@@ -211,7 +217,7 @@ __global__ void __launch_bounds__(kThreads) attn_kernel(const __grid_constant__ 
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[vb][i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-  const int nk = p.seq_mode == AV2V_SEQ_ROWS ? p.seq_kv : 1 << 30;
+  const int nk = p.seq_kv;  // rows: keys per key sequence; frames: F (keys past it are zero-filled, and masked here)
   for (int kt = 0; kt < n_kv; ++kt) {
     if (kt + 1 < n_kv) {
       load_kv(kt + 1, (kt + 1) & 1);
@@ -484,6 +490,7 @@ struct TAttnP {
   const __half* wqkv;
   __half* o;
   int ldx, ldo, F, HW, heads, Cx, ppt, pix_tiles, src_clips;
+  int n_kt;  // key tiles per warpgroup: 1 (its own half) when F | 64, else 2
   float scale_log2;
 };
 
@@ -564,10 +571,12 @@ __global__ void __launch_bounds__(kThreads) tattn_fused_kernel(const __grid_cons
   item /= p.pix_tiles;
   const int h = item % p.heads;
   const int clip = item / p.heads;  // source clip (n_v = 3) or clip
-  const int pix0 = pt * p.ppt, F = p.F, C = p.heads * HD;
+  const int pix0 = pt * p.ppt, F = p.F, C = p.heads * HD, pix_end = min(pix0 + p.ppt, p.HW);
+  // slot i -> (pixel i / F, frame i % F) below pix_end; tail slots (i / F >= ppt) enter the projection as zero rows and are
+  // never stored
   auto row_in = [&](int c, int i) -> long long {
     const int pix = pix0 + i / F;
-    return pix < p.HW ? (static_cast<long long>(c) * F + i % F) * p.HW + pix : -1;
+    return pix < pix_end ? (static_cast<long long>(c) * F + i % F) * p.HW + pix : -1;
   };
   {
     float acc[3][32];
@@ -594,11 +603,12 @@ __global__ void __launch_bounds__(kThreads) tattn_fused_kernel(const __grid_cons
     for (int i = 0; i < 32; ++i) o[b][i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   const int q0 = wg * 64;
-  // sequences of <= 64 frames never cross the 64-slot halves: each warpgroup then needs only its own key half.  The tile index
-  // is data, not control flow, so both warpgroups issue the same wgmma sequence (no divergent path around the wgmma).
-  const int n_kt = F <= 64 ? 1 : 2;
+  // when F divides 64 no pixel crosses the 64-slot halves: each warpgroup then needs only its own key half.  For every other F
+  // some pixel does (e.g. F = 24: slots 48..71), so both warpgroups visit both key tiles.  The tile count is the same for both
+  // and the tile index is data, not control flow, so both issue the same wgmma sequence (no divergent path around the wgmma).
+  const int n_kt = p.n_kt;
   for (int it = 0; it < n_kt; ++it) {
-    const int kt = F <= 64 ? wg : it;
+    const int kt = n_kt == 1 ? wg : it;
     const int k0 = kt * 64;
     uint32_t vt[NV];
 #pragma unroll
@@ -668,8 +678,6 @@ extern "C" int av2v_attn_pnp_f16(const av2v_attn_args* a, av2v_stream_t stream_)
     AV2V_REQUIRE(HW > 0 && a->batch % HW == 0, AV2V_EINVAL, "attn/frames: batch must be clips*HW");
     AV2V_REQUIRE((a->seq_kv <= 0 || a->seq_kv == a->seq) && p.kv_div == 1, AV2V_ENOSUP,
                  "attn/frames: self-attention only (seq_kv / kv_batch_div are rows-mode options)");
-    AV2V_REQUIRE((F <= 128 && 128 % F == 0) || (F % 128 == 0), AV2V_ENOSUP,
-                 "attn/frames: F must divide 128 or be a multiple of 128 (got %d)", F);
     const int clips = a->batch / HW;
     p.F = F;
     p.HW = HW;
@@ -678,7 +686,7 @@ extern "C" int av2v_attn_pnp_f16(const av2v_attn_args* a, av2v_stream_t stream_)
       p.pix_tiles = (HW + p.ppt - 1) / p.ppt;
       items = static_cast<long long>(clips) * a->heads * p.pix_tiles;
     } else {
-      p.f_tiles = F / 128;
+      p.f_tiles = (F + 127) / 128;
       items = static_cast<long long>(clips) * HW * a->heads * p.f_tiles;
     }
   } else {
@@ -722,7 +730,7 @@ extern "C" int av2v_tattn_fused_f16(const av2v_tattn_fused_args* a, av2v_stream_
   AV2V_REQUIRE(a != nullptr, AV2V_EINVAL, "tattn_fused: null args");
   AV2V_REQUIRE(a->x && a->wqkv && a->o, AV2V_EINVAL, "tattn_fused: null x / wqkv / o");
   AV2V_REQUIRE(a->clips > 0 && a->F > 0 && a->HW > 0 && a->heads > 0 && a->Cx > 0, AV2V_EINVAL, "tattn_fused: bad shape");
-  AV2V_REQUIRE(a->F <= 128 && 128 % a->F == 0, AV2V_ENOSUP, "tattn_fused: F must divide 128 (got %d)", a->F);
+  AV2V_REQUIRE(a->F <= 128, AV2V_ENOSUP, "tattn_fused: F must be at most 128 (got %d)", a->F);
   AV2V_REQUIRE(a->Cx % 64 == 0, AV2V_ENOSUP, "tattn_fused: the input width must be a multiple of 64 (got %d)", a->Cx);
   AV2V_REQUIRE(a->ldx % 8 == 0 && a->ldx >= a->Cx && a->ldo % 8 == 0 && a->ldo >= a->heads * HD, AV2V_EINVAL,
                "tattn_fused: row strides must be multiples of 8 covering the rows");
@@ -743,6 +751,7 @@ extern "C" int av2v_tattn_fused_f16(const av2v_tattn_fused_args* a, av2v_stream_
   p.Cx = a->Cx;
   p.ppt = 128 / a->F;
   p.pix_tiles = (a->HW + p.ppt - 1) / p.ppt;
+  p.n_kt = 64 % a->F == 0 ? 1 : 2;
   p.src_clips = a->n_v == 3 ? a->clips / 3 : a->clips;
   p.scale_log2 = a->scale * 1.4426950408889634f;
   const long long items = static_cast<long long>(p.src_clips) * a->heads * p.pix_tiles;

@@ -422,7 +422,8 @@ def _reach(t: torch.Tensor, name: str, rows: int, cols: int, offset: int = 0) ->
 def attention(q, k, v, heads: int, seq: int, batch: int, out, scale: float = 0.125, n_v: int = 1,
               v_branch_stride: int = 0, o_branch_stride: int = 0, frames_mode: bool = False, HW: int = 0,
               seq_kv: int = 0, kv_batch_div: int = 0):
-    """PnP self-attention core (pnp_utils.py:189-210 / 295-316). q,k,v,out: 2-D token matrices (row-strided views ok)."""
+    """PnP self-attention core (pnp_utils.py:189-210 / 295-316). q,k,v,out: 2-D token matrices (row-strided views ok).
+    frames_mode: temporal attention over frame-major tokens [batch / HW clips][seq = F frames][HW][*]; any F >= 1."""
     global _launches
     for name, t in (("q", q), ("k", k), ("v", v), ("o", out)):
         _f16_cuda(t, "attention." + name)
@@ -448,7 +449,8 @@ def attention(q, k, v, heads: int, seq: int, batch: int, out, scale: float = 0.1
 
 def temporal_attention_fused(x, wqkv, heads: int, F: int, HW: int, clips: int, out, scale: float = 0.125, n_v: int = 1):
     """Temporal self-attention with the Q/K/V projection fused in (csrc/attention_wgmma.cu; pnp_utils.py:247-334).
-    x: frame-major tokens [clips*F*HW, Cx]; wqkv: [3*heads*64, Cx]; out: [clips*F*HW, heads*64].  n_v = 3: PnP-injected step,
+    x: frame-major tokens [clips*F*HW, Cx]; wqkv: [3*heads*64, Cx]; out: [clips*F*HW, heads*64]; 1 <= F <= 128 (longer clips
+    take ops.linear + ops.attention).  n_v = 3: PnP-injected step,
     clips ordered [source | uncond | cond]; Q, K of every clip come from the source clip of the same index (pnp_utils.py:295-302)."""
     global _launches
     for name, t in (("x", x), ("wqkv", wqkv), ("o", out)):

@@ -161,7 +161,7 @@ class AttnProcessor:
         inject = self.inject_now() and (B % 3 == 0)
         wqkv = attn.fused_qkv_weight()
         out_attn = torch.empty((rows, C), dtype=tokens.dtype, device=tokens.device)
-        fusable = frames_view and 128 % seq == 0 and C % 64 == 0 and wqkv.shape[0] == 3 * heads * 64
+        fusable = frames_view and seq <= 128 and C % 64 == 0 and wqkv.shape[0] == 3 * heads * 64
         if fusable:
             # temporal self-attention: Q/K/V projection fused into the attention kernel (Q, K, V never reach HBM); on injected
             # steps (pnp_utils.py:295-302) Q and K of all three branches are projected from the SOURCE clip inside the kernel

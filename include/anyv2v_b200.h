@@ -183,7 +183,8 @@ int av2v_layernorm_f16(const av2v_layernorm_args* a, av2v_stream_t stream);
  *   - AV2V_SEQ_ROWS (spatial): sequence b = rows [b*seq, (b+1)*seq).
  *   - AV2V_SEQ_FRAMES (temporal): tokens live frame-major as [clips][F][HW][*]; sequence (clip, pixel) =
  *     rows clip*F*HW + f*HW + pixel, f = 0..F-1 (no [B,C,F,h,w]->[B*hw,F,C] transpose is materialised).
- *     `batch` = clips*HW, seq = F (F must divide 128 or be a multiple of 128).
+ *     `batch` = clips*HW, seq = F, any F >= 1.  F <= 128: floor(128 / F) pixels share a CTA (all 128 slots used
+ *     when F divides 128); F > 128: one pixel per CTA, ceil(F / 128) query tiles.
  */
 enum { AV2V_SEQ_ROWS = 0, AV2V_SEQ_FRAMES = 1 };
 typedef struct {
@@ -207,7 +208,7 @@ int av2v_attn_pnp_f16(const av2v_attn_args* a, av2v_stream_t stream);
  * i2vgen-xl/pnp_utils.py:247-334 is the reference's restatement of that processor, ModifiedTmpAttnProcessor).
  * x holds the LayerNorm-ed tokens frame-major as [clips][F][HW][ldx]; wqkv = rows [Wq ; Wk ; Wv], each [heads*64, Cx];
  * o receives softmax(Q K^T * scale) V per (clip, pixel) sequence of F tokens, head h in columns [h*64, h*64+64).
- * F must divide 128, Cx % 64 == 0.  Q, K, V never reach global memory.
+ * 1 <= F <= 128 (floor(128 / F) pixels per CTA), Cx % 64 == 0.  Q, K, V never reach global memory.
  * n_v = 1: plain self-attention.  n_v = 3: the PnP-injected step (pnp_utils.py:295-302) — the `clips` clips are ordered
  * [source | uncond | cond] (clips % 3 == 0); Q and K of every clip are projected from the SOURCE clip of the same index,
  * V from the clip itself: the result the reference gets by overwriting q, k of the uncond / cond chunks.

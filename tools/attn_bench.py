@@ -2,12 +2,18 @@
 48; the injected sites at n_v = 3 over the 16 source sequences) of the bench workload against other builds of the library,
 alternated in one process.
 
-    python tools/attn_bench.py --other path/to/libanyv2v_b200.so [--other ...] [--iters 20] [--rounds 5]
+    python tools/attn_bench.py [--other path/to/libanyv2v_b200.so ...] [--frames F ...] [--iters 20] [--rounds 5]
 
 Each round times every shape with CUDA events on this build and then on each other build; the report gives, per shape, the
 median over rounds of the mean time per call and the achieved TFLOP/s over the FLOPs the kernel needs: 4 * rows * keys * 64
 per head for QK^T and PV, with PV counted once per V branch at n_v = 3 (as bench.attention_roofline counts it), and the share
-of the H100 SXM data-sheet 989 TFLOP/s.  The card name, power limit and SM clock are printed with the numbers."""
+of the H100 SXM data-sheet 989 TFLOP/s.  The card name, power limit and SM clock are printed with the numbers.
+
+--frames adds the fused temporal self-attention (av2v_tattn_fused_f16) of the 64 x 64 level (HW 4096, Cx 320, 5 heads) for
+each frame count F, at n_v = 1 (one clip) and n_v = 3 (three clips, Q / K from the source).  Its FLOPs count only the slots
+that hold a frame, not the empty tail of a CTA's 128 slots: the projections (2 * Cx * 64 per head and row, for Q and K of the
+source rows and V of every row) plus QK^T and PV over the F frames of each pixel.  A build that rejects a case is reported
+as "unsupported"."""
 from __future__ import annotations
 
 import argparse
@@ -27,6 +33,24 @@ from tools.numerics_bench import _card, _load, _time  # noqa: E402
 PEAK_TFLOPS = 989.0
 LEVELS = ((4096, 5), (1024, 10), (256, 20), (64, 20))  # (tokens per frame, heads) of the UNet's spatial transformers
 N_CTX = 145  # text + image context tokens of the cross-attention
+
+
+def _fused_cases(dev, frames):
+    """name -> (fn, flops) of the fused temporal attention at the 64 x 64 level"""
+    HW, Cx, heads = 4096, 320, 5
+    C = heads * 64
+    cases = {}
+    for F in frames:
+        for nv in (1, 3):
+            rows = nv * F * HW
+            x = torch.randn(rows, Cx, device=dev).half()
+            w = (torch.randn(3 * C, Cx, device=dev) * Cx ** -0.5).half()
+            o = torch.empty(rows, C, device=dev).half()
+            src = F * HW  # rows of the source clip (the only clip at n_v = 1)
+            flops = 2 * Cx * C * (2 * src + rows) + 2 * (1 + nv) * HW * heads * F * F * 64
+            cases[f"fused temporal F={F:3d} 4096x{heads} nv{nv}"] = (
+                lambda x=x, w=w, o=o, F=F, nv=nv: ops.temporal_attention_fused(x, w, heads, F, HW, nv, o, n_v=nv), flops)
+    return cases
 
 
 def _cases(dev):
@@ -59,7 +83,8 @@ def _cases(dev):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--other", action="append", required=True, help="another build of libanyv2v_b200.so (repeatable)")
+    ap.add_argument("--other", action="append", default=[], help="another build of libanyv2v_b200.so (repeatable)")
+    ap.add_argument("--frames", type=int, nargs="*", default=[], help="frame counts of the fused temporal attention cases")
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=5)
     args = ap.parse_args()
@@ -68,16 +93,22 @@ def main():
     libs = {"this": _lib.lib()}
     for path in args.other:
         libs[path] = _load(os.path.abspath(path))
-    cases = _cases("cuda")
+    cases = {**_cases("cuda"), **_fused_cases("cuda", args.frames)}
     times = {(lib, c): [] for lib in libs for c in cases}
-    for lib in libs.values():  # warm-up: module load, first launches
+    unsupported = set()
+    for name, lib in libs.items():  # warm-up: module load, first launches
         _lib._lib = lib
-        for fn, _ in cases.values():
-            fn()
+        for c, (fn, _) in cases.items():
+            try:
+                fn()
+            except _lib.Av2vError:
+                unsupported.add((name, c))
     torch.cuda.synchronize()
     for _ in range(args.rounds):
         for c, (fn, _) in cases.items():
             for name, lib in libs.items():
+                if (name, c) in unsupported:
+                    continue
                 _lib._lib = lib
                 times[(name, c)].append(_time(fn, args.iters))
     _lib._lib = libs["this"]
@@ -89,6 +120,10 @@ def main():
         row = dict(case=c, gflop=round(flops / 1e9, 2))
         line = f"{c:34s}"
         for name in libs:
+            if (name, c) in unsupported:
+                row[tag(name)] = "unsupported"
+                line += f" | {tag(name)} unsupported"
+                continue
             t = statistics.median(times[(name, c)])
             total[name] += t
             row[tag(name)] = dict(us=round(t, 2), tflops=round(flops / t / 1e6, 1))

@@ -106,22 +106,101 @@ def simulate_tile_handoff(rng: random.Random, barrier: bool = True, n_wg: int = 
 
 
 # ---------------------------------------------------------------------------------------------------------- fused key tiles
-def fused_key_tiles(F: int, wg: int, wrong: bool = False):
-    """key tiles (64 slots each) the warpgroup wg visits in tattn_fused_kernel, as in the kernel: kt = wg when F <= 64 (a
-    sequence never crosses the 64-slot halves), else both"""
-    if F <= 64:
+def fused_key_tiles(F: int, wg: int, wrong: bool = False, old_rule: bool = False):
+    """key tiles (64 slots each) the warpgroup wg visits in tattn_fused_kernel, as in the kernel: kt = wg when F divides 64 (no
+    pixel crosses the 64-slot halves), else both.  old_rule: kt = wg for every F <= 64, right only when F divides 128"""
+    if (F <= 64) if old_rule else (64 % F == 0):
         return [1 - wg if wrong else wg]
     return [0, 1]
 
 
-def check_fused_key_tiles(F: int, wrong: bool = False):
-    """every key of a query slot's own pixel (slot // F equal) lies in a visited tile, and the kept keys per row are exactly F"""
+def check_fused_key_tiles(F: int, wrong: bool = False, old_rule: bool = False):
+    """every key of a query slot's own pixel (slot // F equal) lies in a visited tile, and the kept keys per row are exactly F;
+    tail slots (slot >= floor(128 / F) * F, never stored) are not checked"""
+    used = 128 // F * F
     for wg in range(2):
-        tiles = fused_key_tiles(F, wg, wrong)
+        tiles = fused_key_tiles(F, wg, wrong, old_rule)
         for r in range(64):
             q = wg * 64 + r
+            if q >= used:
+                continue
             kept = [64 * kt + c for kt in tiles for c in range(64) if q // F == (64 * kt + c) // F]
             assert len(kept) == F and all(k // F == q // F for k in kept), (F, wg, r, len(kept))
+    return True
+
+
+# ---------------------------------------------------------------------------------------------------------- frame slots
+def frame_slot_rules():
+    """checks that attention_wgmma.cu still launches and maps frames-mode work as frame_slot_items restates it"""
+    s = _src("attention_wgmma.cu")
+    for rule in ("p.ppt = 128 / F;", "p.pix_tiles = (HW + p.ppt - 1) / p.ppt;", "p.f_tiles = (F + 127) / 128;",
+                 "n_kv = (p.F + 63) / 64;", "const int pix_end = min(pix0 + p.ppt, p.HW);", "return pix < pix_end ?",
+                 "return f < p.F ?", "return u < p.F ?", "const int nk = p.seq_kv;", "p.n_kt = 64 % a->F == 0 ? 1 : 2;",
+                 "const int kt = n_kt == 1 ? wg : it;", "C = p.heads * HD, pix_end = min(pix0 + p.ppt, p.HW);"):
+        assert rule in s, f"attention_wgmma.cu no longer contains {rule!r}"
+    return True
+
+
+def frame_slot_items(kernel: str, F: int, HW: int, clips: int = 2, tail_masked: bool = True, old_rule: bool = False):
+    """the work items of frames-mode attn_kernel ("attn") or tattn_fused_kernel ("fused", n_v = 1) for `clips` clips of F
+    frames x HW pixels, as the host launches them and the kernel addresses them.  Yields (qrow, krow, keep): qrow[i] the token
+    row query slot i loads and stores (-1: none), krow[u] the row key slot u loads (-1: zero-filled), keep[i, u] the score
+    mask, with the key tiles a query's warpgroup does not visit masked out.  tail_masked=False: slots past floor(128 / F) * F
+    take the next pixel, as when the tail is not masked; old_rule: the fused kernel's kt = wg for every F <= 64."""
+    import numpy as np
+    if kernel == "attn" and F > 128:  # unpacked: one pixel, ceil(F / 128) query tiles, ceil(F / 64) key tiles
+        n_kv = (F + 63) // 64
+        u = np.arange(n_kv * 64)
+        keep_k = u < F
+        for clip in range(clips):
+            for pix in range(HW):
+                for qt in range((F + 127) // 128):
+                    f = qt * 128 + np.arange(128)
+                    qrow = np.where(f < F, (clip * F + f) * HW + pix, -1)
+                    krow = np.where(u < F, (clip * F + u) * HW + pix, -1)
+                    yield qrow, krow, np.broadcast_to(keep_k, (128, n_kv * 64))
+        return
+    assert F <= 128
+    ppt = 128 // F
+    slot = np.arange(128)
+    group = slot // F
+    keep = group[:, None] == group[None, :]
+    if kernel == "fused":
+        n_kt = 1 if ((F <= 64) if old_rule else (64 % F == 0)) else 2
+        for wg in range(2):
+            visited = np.zeros(128, bool)
+            for it in range(n_kt):
+                kt = wg if n_kt == 1 else it
+                visited[kt * 64:(kt + 1) * 64] = True
+            keep[wg * 64:(wg + 1) * 64] &= visited[None, :]
+    for clip in range(clips):
+        for pt in range((HW + ppt - 1) // ppt):
+            pix0 = pt * ppt
+            pix_end = min(pix0 + ppt, HW) if tail_masked else HW
+            pix = pix0 + group
+            rows = np.where(pix < pix_end, (clip * F + slot % F) * HW + pix, -1)
+            yield rows, rows, keep
+
+
+def check_frame_slot_ownership(kernel: str, F: int, HW: int, clips: int = 2, **kw):
+    """every (clip, pixel, frame) row is stored by exactly one work item, and every stored row keeps exactly the F key rows of
+    its own (clip, pixel): none zero-filled, none of another pixel"""
+    import numpy as np
+    stored = np.zeros(clips * F * HW, np.int64)
+    for qrow, krow, keep in frame_slot_items(kernel, F, HW, clips, **kw):
+        q = np.nonzero(qrow >= 0)[0]
+        np.add.at(stored, qrow[q], 1)
+        valid = krow[krow >= 0]
+        assert len(np.unique(valid)) == len(valid)
+        k = keep[q]                                               # [stored rows, key slots]
+        r = qrow[q][:, None]
+        own = (krow[None, :] >= 0) & (krow[None, :] % HW == r % HW) & (krow[None, :] // HW // F == r // HW // F)
+        bad = k & ~own                                            # a kept key that is zero-filled or of another pixel
+        assert not bad.any(), f"{kernel} F={F} HW={HW}: row {int(r[bad.any(1)][0, 0])} keeps a key outside its pixel"
+        n = k.sum(1)
+        assert (n == F).all(), f"{kernel} F={F} HW={HW}: row {int(r[n != F][0, 0])} keeps {int(n[n != F][0])} keys, not {F}"
+    assert (stored == 1).all(), (f"{kernel} F={F} HW={HW}: rows stored {int(stored.min())}..{int(stored.max())} times "
+                                 f"(first bad row {int(np.nonzero(stored != 1)[0][0])})")
     return True
 
 
