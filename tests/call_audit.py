@@ -23,7 +23,9 @@ goes through ``ops.<name>(...)``, so the package itself is untouched.  For each 
                               the filtered skip within the FreeU bound;
 
 4. compares with the op's element-wise bound (tests/ulp_check.py) and records op, argument signature, worst error in fp16
-   ulps and the smallest margin.  Failures are collected, not raised, so that one pass shows every bad call.
+   ulps and the smallest margin.  Failures are collected, not raised, so that one pass shows every bad call.  The same
+   comparisons feed the sums of tests/bias_check.py, per op, so that ``assert_unbiased`` checks the mean error of each op
+   over the whole pass: a store that rounds in one direction stays inside every call's bound but not inside that mean.
 
 ``perturb(op, index, args, out)`` runs after the op and before the check, so a test can corrupt one call's output (the
 negative controls of tests/test_call_audit_cpu.py); ``snapshot_after=True`` takes the snapshots after the call instead of
@@ -33,13 +35,14 @@ from __future__ import annotations
 
 import inspect
 import math
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 
 import torch
 
 import freeu_ref
 import kernel_contracts as kc
 import sampling_ref
+from bias_check import Moments, moments
 from ulp_check import (KAPPA_ATTN, KAPPA_FREEU, KAPPA_GEGLU, KAPPA_GEMM, KAPPA_NORM, cond_attention, cond_conv_abs, cond_freeu,
                        cond_geglu, cond_groupnorm, cond_layernorm, cond_linear, measure, ulp16)
 
@@ -85,6 +88,7 @@ class Record:
     margin: float = 1.0  # min over the compared elements of (bound - err) / bound; < 0 fails
     ok: bool = True
     detail: str = ""
+    bias: Moments = field(default_factory=Moments)  # the element-wise parts' sums of e (bit-exact parts have none)
 
     def line(self):
         return (f"#{self.index} {self.sig} [{self.units}]: worst {self.worst_ulp:.3g} ulp16, margin {self.margin:+.3g}"
@@ -188,6 +192,19 @@ class CallAudit:
         lines += [f"{s:<{w}}  {c:5d}  {u:11.3g}  {m:+10.3g}" for s, (c, u, m) in rows.items()]
         return "\n".join(lines)
 
+    def bias_by_op(self) -> dict:
+        """op -> Moments pooled over every call of the op"""
+        out = {}
+        for r in self.records:
+            out.setdefault(r.op, Moments())
+            out[r.op] += r.bias
+        return out
+
+    def assert_unbiased(self):
+        """every op with element-wise parts: mean error within the bias bound of tests/bias_check.py, with power"""
+        bad = [f"{op}: {mo.line()}: {v}" for op, mo in self.bias_by_op().items() if mo.n_all and (v := mo.verdict())]
+        assert not bad, "mean error of the pass over the bias bound:\n" + "\n".join(bad)
+
     def families(self) -> dict:
         """op -> (calls, worst ulp, smallest margin)"""
         out = {}
@@ -223,6 +240,7 @@ class CallAudit:
             else:
                 what, got, ref, cond, kappa = part
                 m = measure(got, ref, cond, kappa)
+                rec.bias += moments(got, ref, cond, kappa)
                 n = m["n"]
                 m_ulp, m_margin = m["err_ulp"], -m["over_rel"]
                 if m["n_bad"]:

@@ -1,7 +1,8 @@
 """Negative controls of tests/call_audit.py without a GPU: the audit installed over the tiny-config UNet, with the float64
 contracts standing in for the kernels, on one PnP edit step with every injection firing and FreeU on.  The clean step
 passes; a step whose one call is corrupted by the audit's ``perturb`` hook fails at exactly that call; snapshots taken after
-the call instead of before fail the in-place ops; the unit subsets always hold the first and last unit."""
+the call instead of before fail the in-place ops; layernorm outputs rounded toward zero pass every call's bound and fail the
+mean error of the step; the unit subsets always hold the first and last unit."""
 from types import SimpleNamespace
 
 import pytest
@@ -174,6 +175,37 @@ def test_snapshots_taken_after_the_call_fail_the_in_place_ops(contract_ops, monk
     # the clean audit of the same step passes, so the snapshot timing alone makes the difference
     clean, _ = _audited_edit_step(monkeypatch)
     clean.assert_clean()
+
+
+# ------------------------------------------------------------------------------------------------------------- mean error
+def test_clean_step_is_unbiased(contract_ops, monkeypatch):
+    audit, _ = _audited_edit_step(monkeypatch)
+    for op, mo in audit.bias_by_op().items():
+        print(f"{op:26s} {mo.line()}")
+    audit.assert_unbiased()
+
+
+def test_layernorm_rounded_toward_zero_fails_only_the_mean(contract_ops, monkeypatch):
+    """every layernorm output replaced by its float64 contract rounded toward zero (the fp16 output alone can not be
+    re-rounded): each call stays inside its element-wise bound, the mean error of layernorm over the step does not"""
+    import kernel_contracts as kc
+    from bias_check import round_fp16
+    perturbed = []
+
+    def hook(name, index, p, out):
+        if name == "layernorm":
+            ref = kc.layernorm_exact(p["x"], p["gamma"], p["beta"], p["eps"])
+            out.copy_(round_fp16(ref, "zero").view(out.shape))
+            perturbed.append(index)
+
+    audit, _ = _audited_edit_step(monkeypatch, perturb=hook)
+    assert perturbed == [r.index for r in audit.seen("layernorm")] and perturbed
+    audit.assert_clean()
+    with pytest.raises(AssertionError) as e:
+        audit.assert_unbiased()
+    failed = [line.split(":")[0] for line in str(e.value).splitlines()[1:]]
+    assert failed == ["layernorm"], str(e.value)
+    assert "|mean sign(ref) e| over" in str(e.value)
 
 
 # ------------------------------------------------------------------------------------------------------------- subsets

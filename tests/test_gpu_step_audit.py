@@ -1,6 +1,7 @@
 """The production passes under tests/call_audit.py: every kernel call of a full-size inversion step, two PnP edit steps, an
 edit step with FreeU, one image-to-video step at 704 x 1280 and the VAE at 512 x 512, checked element by element against its
-float64 contract at the arguments the model passes.  All passes run eagerly (no CUDA graph: graph replay is tested
+float64 contract at the arguments the model passes, and the mean error of each op over the pass against the bias bound of
+tests/bias_check.py.  All passes run eagerly (no CUDA graph: graph replay is tested
 bit-equal to eager elsewhere).  Each test asserts that every call passed, that every kernel launch was audited, and that
 the intended kinds of call were reached; ``-s`` prints the per-signature table."""
 import time
@@ -48,9 +49,11 @@ class _Pass:
         a = self.audit
         print(f"\n{self.what}: {len(a.records)} audited calls, {a.launches} audited launches, {launches} launches counted, "
               f"{time.perf_counter() - self.t0:.1f} s\n{a.table()}")
+        bias = a.bias_by_op()
         for op, (calls, ulp, margin) in a.families().items():
-            print(f"  {op:26s} {calls:5d} calls  worst {ulp:.3g} ulp16  min margin {margin:+.3g}")
+            print(f"  {op:26s} {calls:5d} calls  worst {ulp:.3g} ulp16  min margin {margin:+.3g}  {bias[op].line()}")
         a.assert_clean()
+        a.assert_unbiased()
         assert a.launches == launches > 0
         return a
 
