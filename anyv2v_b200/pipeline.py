@@ -71,6 +71,22 @@ class _GraphedIteration:
         self.graph.replay()
 
 
+def _loop_state(latents, timesteps, scheduler, guidance_scale: float, device, eta: float = 0.0,
+                **fields) -> SimpleNamespace:
+    """What the three sampling loops keep per clip: the latents the steps update in place (a copy: the captured graphs read
+    this tensor for the life of the state), the per-step timestep / scheduler-coefficient tables, the static buffers the
+    step body reads them from, and the loop iterations (``I2VGenXLPipeline._run``) with their shared activation pool."""
+    st = SimpleNamespace(latents=latents.to(device).contiguous().clone(), timesteps=timesteps, scheduler=scheduler, eta=eta,
+                         **fields)
+    st.t_table = torch.tensor(timesteps, device=device, dtype=torch.int64)
+    st.coef_table = scheduler.coefficient_table(timesteps, guidance_scale, device, eta=eta)
+    st.g_t = torch.zeros(1, device=device, dtype=torch.int64)
+    st.g_coef = torch.zeros(st.coef_table.shape[-1], device=device, dtype=torch.float32)
+    st.iterations = {}  # graph key of the loop -> _GraphedIteration
+    st.graph_pool = torch.cuda.graph_pool_handle() if st.latents.is_cuda else None
+    return st
+
+
 def tensor2vid(video: torch.Tensor, output_type: str = "np"):
     """pipeline_i2vgen_xl.py:79-97 with diffusers' `VaeImageProcessor.postprocess` (do_normalize=True) inlined:
     video [b, 3, f, H, W] in [-1, 1] -> "pt": [b, f, 3, H, W] in [0, 1]; "np": float32 [b, f, H, W, 3]; "pil": list (per
@@ -173,6 +189,21 @@ class I2VGenXLPipeline:
             width, height = image.size
         return height, width
 
+    def _encode(self, prompt, negative_prompt, image, height, width, num_frames, generator, need_negative: bool,
+                prompt_embeds=None, negative_prompt_embeds=None, image_embeddings=None, image_latents=None):
+        """-> (prompt_embeds, negative_prompt_embeds, image_embeddings, image_latents), each encoded from the raw input
+        unless given.  The negative prompt ("" when None, :348-352) is encoded only when ``need_negative``; ``generator``
+        samples the first-frame VAE latent."""
+        if prompt_embeds is None and prompt is not None:
+            prompt_embeds = self.encode_prompt(prompt)
+        if need_negative and negative_prompt_embeds is None:
+            negative_prompt_embeds = self.encode_prompt(negative_prompt if negative_prompt is not None else "")
+        if image is not None and (image_embeddings is None or image_latents is None):
+            emb, lat = self.encode_first_frame(image, *self._size_of(image, height, width), num_frames, generator)
+            image_embeddings = emb if image_embeddings is None else image_embeddings
+            image_latents = lat if image_latents is None else image_latents
+        return prompt_embeds, negative_prompt_embeds, image_embeddings, image_latents
+
     def enable_freeu(self, s1: float, s2: float, b1: float, b2: float):
         """FreeU (arXiv:2309.11497), pipeline_i2vgen_xl.py:623-650: forwarded to ``unet.enable_freeu``.  s1 / s2 scale the low
         frequencies of the skip features of up blocks 0 / 1, b1 / b2 the first half of their backbone channels.  Applies to
@@ -214,6 +245,39 @@ class I2VGenXLPipeline:
                         return True
         return False
 
+    # -- what the three loops share ----------------------------------------------------------------------------------
+    def _run(self, st, i: int, key, make_body):
+        """Step i's timestep and scheduler coefficients into the static buffers, then the loop iteration for ``key`` (what
+        the captured graph bakes in: hook flags, FreeU setting ...; its body from ``make_body()`` on first use), replayed
+        as a CUDA graph unless ``use_cuda_graphs`` is off."""
+        st.g_t.copy_(st.t_table[i:i + 1])
+        st.g_coef.copy_(st.coef_table[i])
+        it = st.iterations.get(key)
+        if it is None:
+            it = st.iterations[key] = _GraphedIteration(make_body(), on_cuda=st.latents.is_cuda, pool=st.graph_pool)
+        if self.use_cuda_graphs:
+            it.run()
+        else:
+            it.body()
+        return st.latents
+
+    @staticmethod
+    def _loop(st, step, callback, max_steps):
+        """``step(st, i)`` for the first ``max_steps`` timesteps (all by default), each followed by ``callback(i, t, latents)``."""
+        n = len(st.timesteps) if max_steps is None else min(max_steps, len(st.timesteps))
+        for i in range(n):
+            step(st, i)
+            if callback is not None:
+                callback(i, st.timesteps[i], st.latents)
+
+    def _output(self, latents, output_type, return_dict, decode_chunk_size):
+        """"latent" -> the latents; "pt" / "np" / "pil" -> the video decoded by the attached VAE."""
+        if output_type == "latent":
+            frames = latents
+        else:
+            frames = tensor2vid(self.decode_latents(latents, decode_chunk_size=decode_chunk_size), output_type)
+        return SimpleNamespace(frames=frames) if return_dict else (frames,)
+
     # -- image-to-video sampling (pipeline :652-890) ------------------------------------------------------------------
     @torch.no_grad()
     def __call__(self, prompt=None, image=None, height: Optional[int] = 704, width: Optional[int] = 1280,
@@ -249,30 +313,18 @@ class I2VGenXLPipeline:
             if eta > 0 and len(generator) > 1:  # the reference's step noise would index the list per frame (:868)
                 raise ValueError("eta > 0 draws the step noise from one generator: pass a single torch.Generator")
         self._guidance_scale = guidance_scale
-        if prompt_embeds is None and prompt is not None:
-            prompt_embeds = self.encode_prompt(prompt)
-        if (self.do_classifier_free_guidance and negative_prompt_embeds is None
-                and (negative_prompt is not None or prompt is not None)):
-            negative_prompt_embeds = self.encode_prompt(negative_prompt if negative_prompt is not None else "")
-        if image is not None and (image_embeddings is None or image_latents is None):
-            # the reference samples the first-frame latent with the global RNG (:540 passes no generator)
-            emb, lat = self.encode_first_frame(image, height, width, num_frames, generator=None)
-            image_embeddings = emb if image_embeddings is None else image_embeddings
-            image_latents = lat if image_latents is None else image_latents
+        # the reference samples the first-frame latent with the global RNG (:540 passes no generator)
+        prompt_embeds, negative_prompt_embeds, image_embeddings, image_latents = self._encode(
+            prompt, negative_prompt, image, height, width, num_frames, None,
+            self.do_classifier_free_guidance and (negative_prompt is not None or prompt is not None),
+            prompt_embeds, negative_prompt_embeds, image_embeddings, image_latents)
         if latents is None and prompt_embeds is not None and image_latents is not None:  # prepare_latents :595-621
             shape = (n_videos, self.unet.config["in_channels"], num_frames) + tuple(image_latents.shape[-2:])
             latents = randn_tensor(shape, generator=generator, device=self.device, dtype=prompt_embeds.dtype)
         st = self.prepare_call(latents, prompt_embeds, image_latents, image_embeddings, target_fps, num_inference_steps,
                                guidance_scale, negative_prompt_embeds, eta, generator, ddim_init_latents_t_idx)
-        n = len(st.timesteps) if max_steps is None else min(max_steps, len(st.timesteps))
-        for i in range(n):
-            self.call_step(st, i)
-            if callback is not None:
-                callback(i, st.timesteps[i], st.latents)
-        if output_type == "latent":
-            return SimpleNamespace(frames=st.latents) if return_dict else (st.latents,)
-        video = tensor2vid(self.decode_latents(st.latents, decode_chunk_size=decode_chunk_size), output_type)
-        return SimpleNamespace(frames=video) if return_dict else (video,)
+        self._loop(st, self.call_step, callback, max_steps)
+        return self._output(st.latents, output_type, return_dict, decode_chunk_size)
 
     def prepare_call(self, latents, prompt_embeds, image_latents, image_embeddings, target_fps=16, num_inference_steps=50,
                      guidance_scale=9.0, negative_prompt_embeds=None, eta=0.0, generator=None, ddim_init_latents_t_idx=1):
@@ -306,12 +358,8 @@ class I2VGenXLPipeline:
         self.scheduler.timesteps = self.scheduler.timesteps[ddim_init_latents_t_idx:]
         ts = self.scheduler.timesteps.tolist()
         logger.info("Sampling starts from latents_at_t=%s", ts[0] if ts else None)
-        st = SimpleNamespace(latents=latents.to(dev).contiguous().clone(), cond=cond, timesteps=ts, eta=float(eta),
-                             generator=generator, scheduler=self.scheduler, n_videos=n_videos)
-        st.t_table = torch.tensor(ts, device=dev, dtype=torch.int64)
-        st.coef_table = self.scheduler.coefficient_table(ts, guidance_scale if cfg else 1.0, dev, eta=st.eta)
-        st.g_t = torch.zeros(1, device=dev, dtype=torch.int64)
-        st.g_coef = torch.zeros(st.coef_table.shape[1], device=dev, dtype=torch.float32)
+        st = _loop_state(latents, ts, self.scheduler, guidance_scale if cfg else 1.0, dev, eta=float(eta), cond=cond,
+                         generator=generator, n_videos=n_videos)
         st.g_noise = torch.zeros_like(st.latents) if st.eta > 0 else None
         # uncond and cond of one video have the same latents, image latents, fps and timestep: they share the UNet prefix
         # up to the first cross-attention.  With N > 1 the last two branches are different videos.
@@ -329,8 +377,6 @@ class I2VGenXLPipeline:
                                   variance_noise=st.g_noise)
 
         st.body = body
-        st.iterations = {}  # (FreeU setting, eta > 0) -> _GraphedIteration
-        st.graph_pool = torch.cuda.graph_pool_handle() if st.latents.is_cuda else None
         return st
 
     def call_step(self, st, i: int):
@@ -341,17 +387,7 @@ class I2VGenXLPipeline:
             n, c, f, h, w = st.latents.shape
             z = randn_tensor((n * f, c, h, w), generator=st.generator, device=st.latents.device, dtype=st.latents.dtype)
             st.g_noise.copy_(z.view(n, f, c, h, w).permute(0, 2, 1, 3, 4))
-        st.g_t.copy_(st.t_table[i:i + 1])
-        st.g_coef.copy_(st.coef_table[i])
-        key = (self.unet.freeu_state(), st.eta > 0)
-        it = st.iterations.get(key)
-        if it is None:
-            it = st.iterations[key] = _GraphedIteration(st.body, on_cuda=st.latents.is_cuda, pool=st.graph_pool)
-        if self.use_cuda_graphs:
-            it.run()
-        else:
-            it.body()
-        return st.latents
+        return self._run(st, i, (self.unet.freeu_state(), st.eta > 0), lambda: st.body)
 
     # -- phase 1 --------------------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -363,25 +399,18 @@ class I2VGenXLPipeline:
                host_resident: bool = False, **_ignored):
         """DDIM inversion x_0 -> x_T (pipeline :1385-1433).  Returns [b, steps, c, f, h, w] in DESCENDING-t order like
         the reference (:1436); every x_t is kept in ``self.latent_store`` (and written as ddim_latents_{t}.pt)."""
-        if prompt_embeds is None and prompt is not None:
-            prompt_embeds = self.encode_prompt(prompt)
-        if guidance_scale > 1 and negative_prompt_embeds is None:
-            negative_prompt_embeds = self.encode_prompt(negative_prompt if negative_prompt is not None else "")  # :348-352
-        if image is not None and (image_embeddings is None or image_latents is None):
-            height, width = self._size_of(image, height, width)
-            emb, lat = self.encode_first_frame(image, height, width, num_frames)
-            image_embeddings = emb if image_embeddings is None else image_embeddings
-            image_latents = lat if image_latents is None else image_latents
+        prompt_embeds, negative_prompt_embeds, image_embeddings, image_latents = self._encode(
+            prompt, negative_prompt, image, height, width, num_frames, None, guidance_scale > 1,
+            prompt_embeds, negative_prompt_embeds, image_embeddings, image_latents)
         st = self.prepare_invert(latents, prompt_embeds, image_latents, image_embeddings, target_fps,
                                  num_inference_steps, guidance_scale, output_dir, write_files, host_resident,
                                  negative_prompt_embeds=negative_prompt_embeds)
-        n = len(st.timesteps) if max_steps is None else min(max_steps, len(st.timesteps))
         inverted = []
-        for i in range(n):
+
+        def step(st, i):
             self.invert_step(st, i)
             inverted.append(st.store.get(st.timesteps[i], device=st.latents.device))
-            if callback is not None:
-                callback(i, st.timesteps[i], st.latents)
+        self._loop(st, step, callback, max_steps)
         st.store.flush()
         stacked = torch.stack(list(reversed(inverted)), 1)
         return SimpleNamespace(frames=stacked) if return_dict else stacked
@@ -398,7 +427,6 @@ class I2VGenXLPipeline:
         if cfg and negative_prompt_embeds is None:
             raise ValueError("`negative_prompt_embeds` (or a `negative_prompt` string + encoders) is required when guidance_scale > 1")
         dev = self.device
-        latents = latents.to(dev)
         if cfg and latents.shape[0] != 1:
             raise ValueError("inversion with guidance handles one clip per call (the reference's batch is always 1, :571)")
         d = lambda x: x.to(dev)
@@ -414,11 +442,7 @@ class I2VGenXLPipeline:
         ts = self.scheduler.timesteps.tolist()
         store = LatentStore(output_dir, write_files=write_files, host_resident=host_resident)
         self.latent_store = store
-        st = SimpleNamespace(latents=latents.contiguous().clone(), cond=cond, timesteps=ts, store=store, scheduler=self.scheduler)
-        st.t_table = torch.tensor(ts, device=dev, dtype=torch.int64)
-        st.coef_table = self.scheduler.coefficient_table(ts, guidance_scale if cfg else 1.0, dev)
-        st.g_t = torch.zeros(1, device=dev, dtype=torch.int64)
-        st.g_coef = torch.zeros(5, device=dev, dtype=torch.float32)
+        st = _loop_state(latents, ts, self.scheduler, guidance_scale if cfg else 1.0, dev, cond=cond, store=store)
 
         if cfg:
             def body():
@@ -430,24 +454,12 @@ class I2VGenXLPipeline:
                 st.scheduler.step(v, None, st.latents, out=st.latents, coef_dev=st.g_coef)  # in place: x_t -> x_{t+1}
 
         st.body = body
-        st.iterations = {}  # FreeU setting -> _GraphedIteration
-        st.graph_pool = torch.cuda.graph_pool_handle() if st.latents.is_cuda else None
         return st
 
     def invert_step(self, st, i: int):
         """One iteration of the inversion loop (pipeline :1385-1433): UNet (B = 1) -> inverse DDIM step -> keep x_t."""
-        t = st.timesteps[i]
-        st.g_t.copy_(st.t_table[i:i + 1])
-        st.g_coef.copy_(st.coef_table[i])
-        key = self.unet.freeu_state()
-        it = st.iterations.get(key)
-        if it is None:
-            it = st.iterations[key] = _GraphedIteration(st.body, on_cuda=st.latents.is_cuda, pool=st.graph_pool)
-        if self.use_cuda_graphs:
-            it.run()
-        else:
-            it.body()
-        st.store.put(t, st.latents)
+        self._run(st, i, self.unet.freeu_state(), lambda: st.body)
+        st.store.put(st.timesteps[i], st.latents)
         return st.latents
 
     # -- phase 2 --------------------------------------------------------------------------------------------------
@@ -465,36 +477,22 @@ class I2VGenXLPipeline:
                         decode_chunk_size: Optional[int] = None, **_ignored):
         """PnP edit loop (pipeline :1131-1179) over the branches [source, uncond, cond]; `output_type` "latent" returns
         the latents, "pt" / "np" / "pil" decode them with the attached VAE (:1180-1194)."""
-        # raw inputs (the reference's only interface, :1014-1094) are encoded once per clip when encoders / VAE are attached
-        if prompt_embeds is None and prompt is not None:
-            prompt_embeds = self.encode_prompt(prompt)
-        if negative_prompt_embeds is None and (negative_prompt is not None or prompt is not None):
-            negative_prompt_embeds = self.encode_prompt(negative_prompt if negative_prompt is not None else "")
-        if ddim_inv_prompt_embeds is None and ddim_inv_prompt is not None:
-            ddim_inv_prompt_embeds = self.encode_prompt(ddim_inv_prompt)
-        if image is not None and (image_embeddings is None or image_latents is None):
-            height, width = self._size_of(image, height, width)
-            emb, lat = self.encode_first_frame(image, height, width, num_frames, generator)
-            image_embeddings = emb if image_embeddings is None else image_embeddings
-            image_latents = lat if image_latents is None else image_latents
-        if ddim_inv_1st_frame is not None and (ddim_inv_image_embeddings is None or ddim_inv_image_latents is None):
-            height, width = self._size_of(ddim_inv_1st_frame, height, width)
-            emb, lat = self.encode_first_frame(ddim_inv_1st_frame, height, width, num_frames, generator)
-            ddim_inv_image_embeddings = emb if ddim_inv_image_embeddings is None else ddim_inv_image_embeddings
-            ddim_inv_image_latents = lat if ddim_inv_image_latents is None else ddim_inv_image_latents
+        # raw inputs (the reference's only interface, :1014-1094) are encoded once per clip when encoders / VAE are attached;
+        # the source first frame is cropped to the size of the edited one
+        height, width = self._size_of(image, height, width)
+        prompt_embeds, negative_prompt_embeds, image_embeddings, image_latents = self._encode(
+            prompt, negative_prompt, image, height, width, num_frames, generator,
+            negative_prompt is not None or prompt is not None,
+            prompt_embeds, negative_prompt_embeds, image_embeddings, image_latents)
+        ddim_inv_prompt_embeds, _, ddim_inv_image_embeddings, ddim_inv_image_latents = self._encode(
+            ddim_inv_prompt, None, ddim_inv_1st_frame, height, width, num_frames, generator, False,
+            ddim_inv_prompt_embeds, None, ddim_inv_image_embeddings, ddim_inv_image_latents)
         st = self.prepare_edit(latents, prompt_embeds, negative_prompt_embeds, ddim_inv_prompt_embeds, image_embeddings,
                                image_latents, ddim_inv_image_embeddings, ddim_inv_image_latents, target_fps,
                                num_inference_steps, guidance_scale, ddim_init_latents_t_idx, ddim_inv_latents_path,
                                latent_store, skip_dead_source_branch)
-        n = len(st.timesteps) if max_steps is None else min(max_steps, len(st.timesteps))
-        for i in range(n):
-            self.edit_step(st, i)
-            if callback is not None:
-                callback(i, st.timesteps[i], st.latents)
-        if output_type == "latent":
-            return SimpleNamespace(frames=st.latents) if return_dict else (st.latents,)
-        video = tensor2vid(self.decode_latents(st.latents, decode_chunk_size=decode_chunk_size), output_type)
-        return SimpleNamespace(frames=video) if return_dict else (video,)
+        self._loop(st, self.edit_step, callback, max_steps)
+        return self._output(st.latents, output_type, return_dict, decode_chunk_size)
 
     def prepare_edit(self, latents, prompt_embeds, negative_prompt_embeds, ddim_inv_prompt_embeds, image_embeddings,
                      image_latents, ddim_inv_image_embeddings, ddim_inv_image_latents, target_fps, num_inference_steps,
@@ -537,15 +535,9 @@ class I2VGenXLPipeline:
         cond2 = None
         if skip_dead_source_branch and not all(fires):
             cond2 = {k: v[v.shape[0] // 3:].contiguous() for k, v in cond3.items()}  # every entry is branch-major
-        st = SimpleNamespace(latents=d(latents).contiguous().clone(), cond3=cond3, cond2=cond2, timesteps=ts, store=store,
-                             fires=fires, guidance=guidance_scale, skip=skip_dead_source_branch, scheduler=self.scheduler)
-        st.t_table = torch.tensor(ts, device=dev, dtype=torch.int64)
-        st.coef_table = self.scheduler.coefficient_table(ts, guidance_scale, dev)
-        st.g_t = torch.zeros(1, device=dev, dtype=torch.int64)
-        st.g_coef = torch.zeros(5, device=dev, dtype=torch.float32)
+        st = _loop_state(latents, ts, self.scheduler, guidance_scale, dev, cond3=cond3, cond2=cond2, store=store, fires=fires,
+                         guidance=guidance_scale, skip=skip_dead_source_branch)
         st.g_src = torch.zeros_like(st.latents)
-        st.iterations = {}  # (dead source, hook flags, FreeU setting) -> _GraphedIteration
-        st.graph_pool = torch.cuda.graph_pool_handle() if st.latents.is_cuda else None  # one activation pool for all of them
         # uncond and cond are the same latents + image latents -> they share the UNet prefix up to the first cross-attention
         # (I2VGenXLUNet.forward, shared_edit_prefix); the source branch is dropped after the last injection site that fires in
         # the step (its prediction is discarded, pipeline :1160).  Both leave the result unchanged
@@ -583,30 +575,23 @@ class I2VGenXLPipeline:
         register_time(self, t)
         dead_source = st.skip and not st.fires[i]
         flags = self._hook_flags(t)
-        key = (dead_source, flags, self.unet.freeu_state())
-        it = st.iterations.get(key)
-        if it is None:
+
+        def make_body():
             if dead_source:
                 def body():
                     v = self.unet(torch.cat([st.latents, st.latents]), st.g_t, cond=st.cond2,
                                   shared_edit_prefix=st.shared_prefix)[0]
                     st.scheduler.step(v[0:1], None, st.latents, model_output_cond=v[1:2], out=st.latents, coef_dev=st.g_coef)
-            else:
-                site = self._prune_site(flags) if st.prune_source else None
-                lo = 0 if site is not None else 1  # the pruned forward returns [uncond, cond] only
+                return body
+            site = self._prune_site(flags) if st.prune_source else None
+            lo = 0 if site is not None else 1  # the pruned forward returns [uncond, cond] only
 
-                def body():
-                    v = self.unet(torch.cat([st.g_src, st.latents, st.latents]), st.g_t, cond=st.cond3,
-                                  shared_edit_prefix=st.shared_prefix, prune_source_after=site)[0]
-                    st.scheduler.step(v[lo:lo + 1], None, st.latents, model_output_cond=v[lo + 1:lo + 2], out=st.latents,
-                                      coef_dev=st.g_coef)
-            it = st.iterations[key] = _GraphedIteration(body, on_cuda=st.latents.is_cuda, pool=st.graph_pool)
-        st.g_t.copy_(st.t_table[i:i + 1])
-        st.g_coef.copy_(st.coef_table[i])
+            def body():
+                v = self.unet(torch.cat([st.g_src, st.latents, st.latents]), st.g_t, cond=st.cond3,
+                              shared_edit_prefix=st.shared_prefix, prune_source_after=site)[0]
+                st.scheduler.step(v[lo:lo + 1], None, st.latents, model_output_cond=v[lo + 1:lo + 2], out=st.latents,
+                                  coef_dev=st.g_coef)
+            return body
         if not dead_source:
             st.g_src.copy_(st.store.get(t, device=st.latents.device), non_blocking=True)
-        if self.use_cuda_graphs:
-            it.run()
-        else:
-            it.body()
-        return st.latents
+        return self._run(st, i, (dead_source, flags, self.unet.freeu_state()), make_body)

@@ -21,7 +21,7 @@ import torch
 
 from .config import OmegaConf
 from .pipeline import I2VGenXLPipeline
-from .run_group_pnp_edit import _model_dir, build_pipeline, load_source_frames, seed_everything, synthetic_conditioning
+from .run_group_pnp_edit import build_pipeline, load_source_frames, run_sharded, seed_everything, synthetic_conditioning
 from .schedulers import DDIMInverseScheduler, DDIMScheduler
 
 logger = logging.getLogger(__name__)
@@ -69,27 +69,17 @@ def ddim_sampling(config, first_frame, ddim_latents_path, pipe, ddim_scheduler, 
 
 
 def main(template_config, configs_list, device, unet_config=None, pipeline_kwargs=None):
-    from . import distributed
-    rank, world = distributed.rank_world()
-    active = [e for e in configs_list if e.get("active", True)]
-    need_real = any(not OmegaConf.merge(template_config, OmegaConf.create(e)).get("synthetic", False) for e in active)
-    pipe = build_pipeline(device, unet_config, seed=template_config.seed, with_encoders=need_real,
-                          model_dir=_model_dir(template_config), **(pipeline_kwargs or {}))
+    assert len(configs_list) > 0
     g = torch.Generator(device=device).manual_seed(template_config.seed)
     inverse_scheduler = DDIMInverseScheduler.from_pretrained("ali-vilab/i2vgen-xl", subfolder="scheduler")
     ddim_scheduler = DDIMScheduler.from_pretrained("ali-vilab/i2vgen-xl", subfolder="scheduler")
-    assert len(configs_list) > 0
-    out = []
-    for i, entry in enumerate(active):
-        if i % world != rank:
-            continue
-        logger.info("Processing config_entry: %s", entry)
-        config = OmegaConf.merge(template_config, OmegaConf.create(entry))
+
+    def run_entry(pipe, config, i):
         config.video_path = os.path.join(config.video_dir, config.video_name + ".mp4")
         config.video_frames_path = os.path.join(config.video_dir, config.video_name)
         if os.path.exists(config.output_dir) and not config.get("force_recompute_latents", False):
             logger.info("= Inverted latents already exist at %s. Skip.", config.output_dir)
-            continue
+            return None
         if config.get("synthetic", False):
             h, w = config.image_size[1] // 8, config.image_size[0] // 8
             cond = synthetic_conditioning(config.n_frames, h, w, pipe.unet.config["cross_attention_dim"], config.seed + i, device)
@@ -113,7 +103,6 @@ def main(template_config, configs_list, device, unet_config=None, pipeline_kwarg
                 logger.info("### Inverse a null image!")
                 first_frame = Image.new("RGB", (config.image_size[0], config.image_size[1]), (0, 0, 0))
             inv = ddim_inversion(config.inverse_config, first_frame, frame_list, pipe, inverse_scheduler, g)
-        out.append(inv)
         rc = config.recon_config
         if rc.enable_recon:
             rec, frames = ddim_sampling(rc, None if cond is not None else first_frame, rc.ddim_latents_path, pipe,
@@ -128,7 +117,8 @@ def main(template_config, configs_list, device, unet_config=None, pipeline_kwarg
                 image_io.export_to_video(frames, os.path.join(config.output_dir, "ddim_reconstruction.mp4"), fps=10)
                 image_io.export_to_gif(frames, os.path.join(config.output_dir, "ddim_reconstruction.gif"))
                 logger.info("Saved reconstructed video to %s", config.output_dir)
-    return out
+        return inv
+    return run_sharded(build_pipeline, template_config, configs_list, device, run_entry, unet_config, pipeline_kwargs)
 
 
 def cli(argv=None):

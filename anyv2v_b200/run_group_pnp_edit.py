@@ -96,6 +96,21 @@ def load_source_frames(config):
     return frame_list
 
 
+def start_latents(pipe, ddim_scheduler, config, device):
+    """reference :113-132: x_t at ``ddim_init_latents_t_idx`` blended with ``random_ratio`` of noise from the global RNG,
+    then the PnP hooks (:35-48) and the edit scheduler registered on the pipeline."""
+    ddim_scheduler.set_timesteps(config.n_steps)
+    logger.info("ddim_scheduler.timesteps: %s", ddim_scheduler.timesteps)
+    t0 = int(ddim_scheduler.timesteps[config.ddim_init_latents_t_idx])
+    ddim_latents_at_t = load_ddim_latents_at_t(t0, config.ddim_latents_path, map_location=device)
+    random_latents = torch.randn_like(ddim_latents_at_t)
+    logger.info("Blending random_ratio (1 means random latent): %s", config.random_ratio)
+    mixed = random_latents * config.random_ratio + ddim_latents_at_t * (1 - config.random_ratio)
+    init_pnp(pipe, ddim_scheduler, config)
+    pipe.register_modules(scheduler=ddim_scheduler)
+    return mixed
+
+
 def edit_one(pipe, ddim_scheduler, config, device, rank_seed_offset: int = 0):
     config.video_path = os.path.join(config.video_dir, config.video_name + ".mp4")
     config.video_frames_path = os.path.join(config.video_dir, config.video_name)
@@ -108,26 +123,16 @@ def edit_one(pipe, ddim_scheduler, config, device, rank_seed_offset: int = 0):
     h, w = config.image_size[1] // 8, config.image_size[0] // 8
     cross_dim = pipe.unet.config["cross_attention_dim"]
     cond = synthetic_conditioning(config.n_frames, h, w, cross_dim, config.seed + rank_seed_offset, device)
-
-    ddim_scheduler.set_timesteps(config.n_steps)
-    t_idx = config.ddim_init_latents_t_idx
-    t0 = int(ddim_scheduler.timesteps[t_idx])
+    mixed = start_latents(pipe, ddim_scheduler, config, device)
     store = LatentStore(config.ddim_latents_path, write_files=False)
-    ddim_latents_at_t = load_ddim_latents_at_t(t0, config.ddim_latents_path, map_location=device)
-    random_latents = torch.randn_like(ddim_latents_at_t)
-    logger.info("Blending random_ratio (1 means random latent): %s", config.random_ratio)
-    mixed = random_latents * config.random_ratio + ddim_latents_at_t * (1 - config.random_ratio)
-
-    init_pnp(pipe, ddim_scheduler, config)
-    pipe.register_modules(scheduler=ddim_scheduler)
     out = pipe.sample_with_pnp(
         latents=mixed, prompt_embeds=cond["edit_prompt"], negative_prompt_embeds=cond["neg_prompt"],
         ddim_inv_prompt_embeds=cond["inv_prompt"], image_embeddings=cond["edit_image_emb"],
         image_latents=cond["edit_image_latents"], ddim_inv_image_embeddings=cond["src_image_emb"],
         ddim_inv_image_latents=cond["src_image_latents"], num_frames=config.n_frames,
         num_inference_steps=config.n_steps, guidance_scale=config.cfg, target_fps=config.target_fps,
-        ddim_init_latents_t_idx=t_idx, ddim_inv_latents_path=config.ddim_latents_path, latent_store=store,
-        output_type="latent").frames
+        ddim_init_latents_t_idx=config.ddim_init_latents_t_idx, ddim_inv_latents_path=config.ddim_latents_path,
+        latent_store=store, output_type="latent").frames
     output_dir = os.path.join(config.output_dir, config_suffix(config))
     os.makedirs(output_dir, exist_ok=True)
     torch.save(out.cpu(), os.path.join(output_dir, "edited_latents.pt"))
@@ -146,21 +151,14 @@ def edit_one_real(pipe, ddim_scheduler, config, device):
     src_frame_list = load_source_frames(config)
     src_1st_frame = src_frame_list[0]
     edited_1st_frame = image_io.load_image(config.edited_first_frame_path).resize(size, resample=Image.Resampling.LANCZOS)
-    t_idx = config.ddim_init_latents_t_idx
-    ddim_scheduler.set_timesteps(config.n_steps)
-    logger.info("ddim_scheduler.timesteps: %s", ddim_scheduler.timesteps)
-    ddim_latents_at_t = load_ddim_latents_at_t(int(ddim_scheduler.timesteps[t_idx]), config.ddim_latents_path, map_location=device)
-    random_latents = torch.randn_like(ddim_latents_at_t)
-    logger.info("Blending random_ratio (1 means random latent): %s", config.random_ratio)
-    mixed = random_latents * config.random_ratio + ddim_latents_at_t * (1 - config.random_ratio)
-    init_pnp(pipe, ddim_scheduler, config)
-    pipe.register_modules(scheduler=ddim_scheduler)
+    mixed = start_latents(pipe, ddim_scheduler, config, device)
     latents = pipe.sample_with_pnp(
         prompt=config.editing_prompt, image=edited_1st_frame, height=size[1], width=size[0], num_frames=config.n_frames,
         num_inference_steps=config.n_steps, guidance_scale=config.cfg, negative_prompt=config.editing_negative_prompt,
         target_fps=config.target_fps, latents=mixed, generator=torch.Generator(device=device).manual_seed(config.seed),
-        return_dict=True, ddim_init_latents_t_idx=t_idx, ddim_inv_latents_path=config.ddim_latents_path,
-        ddim_inv_prompt=config.ddim_inv_prompt, ddim_inv_1st_frame=src_1st_frame, output_type="latent").frames
+        return_dict=True, ddim_init_latents_t_idx=config.ddim_init_latents_t_idx,
+        ddim_inv_latents_path=config.ddim_latents_path, ddim_inv_prompt=config.ddim_inv_prompt,
+        ddim_inv_1st_frame=src_1st_frame, output_type="latent").frames
     video = pipe.decode_latents(latents)                                  # [1, 3, f, H, W] in [-1, 1]
     frames = image_io.frames_to_pil(video[0].permute(1, 0, 2, 3))
     output_dir = os.path.join(config.output_dir, config_suffix(config))
@@ -242,14 +240,17 @@ def _model_dir(template_config):
     return None
 
 
-def main(template_config, configs_list, device, unet_config=None, pipeline_kwargs=None):
+def run_sharded(build, template_config, configs_list, device, run_entry, unet_config=None, pipeline_kwargs=None):
+    """The group loop of both runners (reference :74-81): one pipeline from ``build`` (``build_pipeline`` as the calling
+    runner module names it, so either runner's builder can be replaced on its own) for every entry, with the CLIP towers
+    and the VAE when any active entry takes real inputs, and ``run_entry(pipe, config, i)`` on the template merged with the
+    i-th active entry.  Entry i runs on rank i % world.  Returns the results that are not None."""
     from . import distributed
     rank, world = distributed.rank_world()
     active = [e for e in configs_list if e.get("active", True)]
     need_real = any(not OmegaConf.merge(template_config, OmegaConf.create(e)).get("synthetic", False) for e in active)
-    pipe = build_pipeline(device, unet_config, seed=template_config.seed, with_encoders=need_real,
-                          model_dir=_model_dir(template_config), **(pipeline_kwargs or {}))
-    ddim_scheduler = DDIMScheduler.from_pretrained("ali-vilab/i2vgen-xl", subfolder="scheduler")
+    pipe = build(device, unet_config, seed=template_config.seed, with_encoders=need_real,
+                 model_dir=_model_dir(template_config), **(pipeline_kwargs or {}))
     for e in configs_list:
         if not e.get("active", True):
             logger.info("Skipping config_entry: %s", e)
@@ -258,9 +259,17 @@ def main(template_config, configs_list, device, unet_config=None, pipeline_kwarg
         if i % world != rank:  # clips shard one-per-GPU; no data-path collective (SURVEY 8e)
             continue
         logger.info("Processing config_entry: %s", entry)
-        config = OmegaConf.merge(template_config, OmegaConf.create(entry))
-        results.append(edit_one(pipe, ddim_scheduler, config, device, rank_seed_offset=i))
+        out = run_entry(pipe, OmegaConf.merge(template_config, OmegaConf.create(entry)), i)
+        if out is not None:
+            results.append(out)
     return results
+
+
+def main(template_config, configs_list, device, unet_config=None, pipeline_kwargs=None):
+    ddim_scheduler = DDIMScheduler.from_pretrained("ali-vilab/i2vgen-xl", subfolder="scheduler")
+    return run_sharded(build_pipeline, template_config, configs_list, device,
+                       lambda pipe, config, i: edit_one(pipe, ddim_scheduler, config, device, rank_seed_offset=i),
+                       unet_config, pipeline_kwargs)
 
 
 def cli(argv=None):
