@@ -14,8 +14,20 @@
 // Two CTAs per SM (2 x 97 KB of shared memory, <= 128 registers per thread): one CTA's prologue loads, K-loop gathers and
 // epilogue run while the other's wgmma keep the tensor cores busy.  A tile's K loop is short (5 blocks at K = 320), so
 // this overlap between tiles is worth more than a deeper ring inside one: with 4 stages only one CTA fits.
-// Epilogue from the accumulator registers: + bias / rowbias / residual per slot, fp16 pairs stored directly; GEGLU pairs the
-// h and gate columns (blocks of 32, interleaved by geglu_pack) which the accumulator layout puts in the same thread.
+// Epilogue through shared memory, each warp on its own 16 rows of the tile (the rows its accumulators hold), so it needs no
+// block barrier: + bias / rowbias in the registers, then per slot + residual, fp16 pairs written in accumulator order to a
+// 128 x 128 staging tile (256-byte rows, 16-byte chunk c of row r at chunk c ^ (r & 7): the 8 rows x 4 lanes of a fragment
+// store and the 8 chunks a quarter warp copies out both cover the 32 banks once), __syncwarp, and the warp copies its rows
+// out with 16-byte stores, consecutive lanes on consecutive chunks of one output row (whole 128-byte lines; N, ldo and
+// slot_stride are multiples of 8, so every chunk is whole: stored iff its row < M and its first column < N).  The tile
+// takes the ring slot that block num_kb - 3 left, free from the top of the last K block, and the residual tile of slot 0 is
+// fetched there by cp.async as soon as the last wgmma are issued, so it lands under them; each warp fetches the chunks it
+// will itself consume.  (Issued from inside the K loop, ptxas serializes the wgmma.)  The residual tiles of further slots go
+// to the other two ring slots once every warpgroup has retired its wgmma.  A value is
+// rounded once: the fp32 sum of accumulator and residual is what gets packed, over the residual's place in the tile.  All
+// of a warp's residual reads complete before its first store, so a residual that aliases out stays safe.  GEGLU pairs the
+// h and gate columns (blocks of 32, interleaved by geglu_pack) which the accumulator layout puts in the same thread; its
+// output tile is 128 x 64.
 #include "host_util.cuh"
 #include "ptx.cuh"
 
@@ -149,6 +161,32 @@ __device__ __forceinline__ void load_stage(const GemmP& p, const ARows& ar, int 
   }
 }
 
+// ---- epilogue staging tile: one ring slot (2 * kTileBytes = 128 rows x 256 bytes), XOR-swizzled like the operand tiles
+__device__ __forceinline__ uint32_t stage_offset(int row, int chunk) {
+  return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));
+}
+
+// element offset of output row m inside a slot of out / residual
+__device__ __forceinline__ long long out_row_offset(const GemmP& p, int m) {
+  if (!p.up2) return static_cast<long long>(m) * p.ldo;
+  // low-resolution pixel (n, i, j) -> (n, 2 i + py, 2 j + px) of the [NF][2H][2W] output
+  const int j = m % p.Wo, t = m / p.Wo, i = t % p.Ho, n = t / p.Ho;
+  return ((static_cast<long long>(n) * 2 * p.Ho + 2 * i + p.py) * (2 * p.Wo) + 2 * j + p.px) * p.ldo;
+}
+
+// This warp's 16 rows of the residual tile of `slot` -> staging tile: per instruction 2 rows x 16 chunks, zero-filled past M / N
+__device__ __forceinline__ void load_residual_rows(const GemmP& p, int slot, int m0, int n0, uint32_t tile) {
+  const int lane = threadIdx.x & 31, ch = lane & 15;
+  const int c = n0 + 8 * ch;
+  const __half* src = p.residual + slot * p.slot_stride + c;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int r = (threadIdx.x >> 5) * 16 + 2 * i + (lane >> 4);
+    const bool v = m0 + r < p.M && c < p.N;
+    cp_async16(tile + stage_offset(r, ch), v ? src + out_row_offset(p, m0 + r) : p.residual, v);
+  }
+}
+
 __global__ void __launch_bounds__(kThreads, 2) gemm_wgmma_kernel(const __grid_constant__ GemmP p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -194,78 +232,103 @@ __global__ void __launch_bounds__(kThreads, 2) gemm_wgmma_kernel(const __grid_co
     wgmma_wait<1>();
     reg_fence(d);
   }
+  // the ring slot block nk - 3 left stays free: the residual tile of slot 0 is fetched there under the last wgmma
+  if (p.residual) load_residual_rows(p, 0, m0, n0, sA(nk % kStages));
   wgmma_wait<0>();
   reg_fence(d);
-  cp_async_wait<0>();
 
-  // ---- epilogue: thread owns rows r, r + 8 and column pairs 8 j + 2 (lane & 3) of its warpgroup's 64 x 128 block
-  const int rbase = m0 + wg * 64 + acc_row(0);
+  // ---- epilogue: thread owns rows r, r + 8 and column pairs 8 j + 2 (lane & 3) of its warp's 16 rows; staging tile of
+  // slot s = ring slot (nk + s) % kStages
+  const int lane = threadIdx.x & 31;
+  const int r0 = wg * 64 + acc_row(0);
   const int cq = 2 * (threadIdx.x & 3);
+  const int n_res = p.residual ? p.n_slots : 1;  // distinct tiles: without a residual every slot stores the same one
+  if (n_res > 1) {
+    __syncthreads();  // the other ring slots held the last operands: every warpgroup has retired its wgmma
+    for (int s = 1; s < n_res; ++s) load_residual_rows(p, s, m0, n0, sA((nk + s) % kStages));
+  }
   if (p.geglu) {
+    const uint32_t tile = sA(nk % kStages);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int m = rbase + 8 * h;
-      if (m >= p.M) continue;
-      __half* orow = p.out + static_cast<long long>(m) * p.ldo;
+    for (int g = 0; g < 2; ++g) {
 #pragma unroll
-      for (int g = 0; g < 2; ++g) {
+      for (int jj = 0; jj < 4; ++jj) {
+        const int jh = 8 * g + jj, jg = jh + 4;
+        const int ch = n0 + 8 * jh + cq, cg = n0 + 8 * jg + cq;
+        if (ch >= p.N) continue;
+        float2 bh = make_float2(0.f, 0.f), bg = bh;
+        if (p.bias) {
+          bh = __half22float2(*reinterpret_cast<const __half2*>(p.bias + ch));
+          bg = __half22float2(*reinterpret_cast<const __half2*>(p.bias + cg));
+        }
 #pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int jh = 8 * g + jj, jg = jh + 4;
-          const int ch = n0 + 8 * jh + cq, cg = n0 + 8 * jg + cq;
-          if (ch >= p.N) continue;
+        for (int h = 0; h < 2; ++h) {
           float h0 = d[4 * jh + 2 * h], h1 = d[4 * jh + 2 * h + 1];
           float g0 = d[4 * jg + 2 * h], g1 = d[4 * jg + 2 * h + 1];
           if (p.bias) {
-            const float2 bh = __half22float2(*reinterpret_cast<const __half2*>(p.bias + ch));
-            const float2 bg = __half22float2(*reinterpret_cast<const __half2*>(p.bias + cg));
             h0 += bh.x; h1 += bh.y; g0 += bg.x; g1 += bg.y;
           }
-          const int oc = n0 / 2 + 32 * g + 8 * jj + cq;
-          *reinterpret_cast<uint32_t*>(orow + oc) = pack_half2(h0 * gelu_erf_fast(g0), h1 * gelu_erf_fast(g1));
+          st_shared_u32(tile + stage_offset(r0 + 8 * h, 4 * g + jj) + 2 * cq,
+                        pack_half2(h0 * gelu_erf_fast(g0), h1 * gelu_erf_fast(g1)));
         }
       }
     }
-    return;
+  } else {
+    const __half* rb[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = m0 + r0 + 8 * h;
+      rb[h] = p.rowbias && m < p.M ? p.rowbias + static_cast<long long>(m / p.rows_per_rowbias) * p.N : nullptr;
+    }
+    cp_async_commit();
+    cp_async_wait<0>();
+    __syncwarp();  // the residual chunks this warp's lanes fetched for each other have landed
+    for (int s = 0; s < n_res; ++s) {
+      const uint32_t tile = sA((nk + s) % kStages);
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int c = n0 + 8 * j + cq;
+        if (c >= p.N) continue;
+        float2 b = make_float2(0.f, 0.f);
+        if (p.bias) b = __half22float2(*reinterpret_cast<const __half2*>(p.bias + c));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t at = tile + stage_offset(r0 + 8 * h, j) + 2 * cq;
+          float o0 = d[4 * j + 2 * h], o1 = d[4 * j + 2 * h + 1];
+          if (p.bias) {
+            o0 += b.x;
+            o1 += b.y;
+          }
+          if (rb[h]) {
+            const float2 t = __half22float2(*reinterpret_cast<const __half2*>(rb[h] + c));
+            o0 += t.x;
+            o1 += t.y;
+          }
+          if (p.residual) {
+            const uint32_t rr = ld_shared_u32(at);
+            const float2 r = __half22float2(*reinterpret_cast<const __half2*>(&rr));
+            o0 += r.x;
+            o1 += r.y;
+          }
+          st_shared_u32(at, pack_half2(o0, o1));
+        }
+      }
+    }
   }
+  __syncwarp();
+
+  // ---- copy-out: lane -> 16-byte chunk of a row, a warp instruction covers 2 rows x 256 bytes (GEGLU: 4 rows x 128 bytes)
+  const int lg = p.geglu ? 3 : 4;  // log2(chunks per output row of the tile)
+  const int col0 = p.geglu ? n0 / 2 : n0, n_out = p.geglu ? p.N / 2 : p.N;
+  for (int s = 0; s < p.n_slots; ++s) {
+    const uint32_t tile = sA((nk + (p.residual ? s : 0)) % kStages);
+    __half* out = p.out + s * p.slot_stride + col0;
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int m = rbase + 8 * h;
-    if (m >= p.M) continue;
-    long long orow;
-    if (p.up2) {  // low-resolution pixel (n, i, j) -> (n, 2 i + py, 2 j + px) of the [NF][2H][2W] output
-      const int j = m % p.Wo, t = m / p.Wo, i = t % p.Ho, n = t / p.Ho;
-      orow = (static_cast<long long>(n) * 2 * p.Ho + 2 * i + p.py) * (2 * p.Wo) + 2 * j + p.px;
-    } else {
-      orow = m;
-    }
-    orow *= p.ldo;
-    const __half* rb = p.rowbias ? p.rowbias + static_cast<long long>(m / p.rows_per_rowbias) * p.N : nullptr;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int c = n0 + 8 * j + cq;
-      if (c >= p.N) continue;
-      float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
-      if (p.bias) {
-        const float2 b = __half22float2(*reinterpret_cast<const __half2*>(p.bias + c));
-        v0 += b.x;
-        v1 += b.y;
-      }
-      if (rb) {
-        const float2 b = __half22float2(*reinterpret_cast<const __half2*>(rb + c));
-        v0 += b.x;
-        v1 += b.y;
-      }
-      for (int s = 0; s < p.n_slots; ++s) {
-        const long long off = s * p.slot_stride + orow + c;
-        float o0 = v0, o1 = v1;
-        if (p.residual) {
-          const float2 r = __half22float2(*reinterpret_cast<const __half2*>(p.residual + off));
-          o0 += r.x;
-          o1 += r.y;
-        }
-        *reinterpret_cast<uint32_t*>(p.out + off) = pack_half2(o0, o1);
-      }
+    for (int i = 0; i < 8; ++i) {
+      const int idx = 32 * i + lane;
+      const int r = (threadIdx.x >> 5) * 16 + (idx >> lg), ch = idx & ((1 << lg) - 1);
+      if ((idx >> lg) < 16 && m0 + r < p.M && col0 + 8 * ch < n_out)
+        st_global_v4(out + out_row_offset(p, m0 + r) + 8 * ch, ld_shared_v4(tile + stage_offset(r, ch)));
     }
   }
 }
@@ -286,6 +349,7 @@ extern "C" int av2v_gemm_f16(const av2v_gemm_args* a, av2v_stream_t stream_) {
   AV2V_REQUIRE((a->geglu || a->ldo >= a->N) && a->ldo % 8 == 0, AV2V_EINVAL,
                "gemm: ldo must be >= N and a multiple of 8");
   AV2V_REQUIRE(a->n_slots >= 1, AV2V_EINVAL, "gemm: n_slots must be >= 1");
+  AV2V_REQUIRE(!a->residual || a->n_slots <= kStages, AV2V_ENOSUP, "gemm: at most %d slots with a residual (one staging tile each)", kStages);
   AV2V_REQUIRE(a->n_slots == 1 || a->slot_stride % 8 == 0, AV2V_EALIGN, "gemm: slot_stride must be a multiple of 8");
   AV2V_REQUIRE(aligned16(a->a) && aligned16(a->w) && aligned16(a->out), AV2V_EALIGN,
                "gemm: a/w/out must be 16-byte aligned");

@@ -92,6 +92,25 @@ __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
+// ------------------------------------------------------------------ shared memory by 32-bit address, 16-byte global store
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+
+__device__ __forceinline__ void st_global_v4(void* p, uint4 v) {  // p 16-byte aligned
+  asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+
 // ------------------------------------------------------------------ 128-byte-swizzled operand tiles
 // A K-major operand tile is rows of 64 fp16 (128 B); the 16-byte chunk c of row r sits at chunk c ^ (r & 7), 8 rows form a
 // 1024-byte swizzle atom.  Tiles must start on a 1024-byte boundary.

@@ -69,8 +69,19 @@ def _cases(dev):
             wc = _w(C, 9 * C, dev)
             cases[f"conv3x3+res {M}x{C}x{9 * C}"] = (lambda xi=xi, w=wc, b=bias, r=res, o=out: ops.conv3x3(xi, w, bias=b, residual=r, out=o),
                                                     2 * M * C * 9 * C, 2 * (M * C + 9 * C * C + 2 * M * C))
+            # linear + bias + a per-frame rowbias (the time-embedding epilogue of a resnet's conv1, on a short K loop)
+            tproj = (torch.randn(B * F, C, device=dev) * 0.5).half()
+            wl = _w(C, C, dev)
+            cases[f"linear+rowbias {M}x{C}x{C}"] = (lambda x=x, w=wl, b=bias, t=tproj, o=out, r=hw * hw: ops.linear(x, w, bias=b, rowbias=t, rows_per_rowbias=r, out=o),
+                                                   2 * M * C * C, 2 * (M * C + C * C + B * F * C + M * C))
+            if B == 3 and lvl == 2:
+                # conv injection of the edit step: conv2 of the source clip, its tile stored to the 3 branch slots, each + its shortcut
+                Ms = F * hw * hw
+                cases[f"conv3x3+res 3 slots {Ms}x{C}x{9 * C}"] = (
+                    lambda xi=xi[:F], w=wc, b=bias, r=res, o=out, s=Ms * C: ops.conv3x3(xi, w, bias=b, residual=r.view(3, -1, r.shape[1]), out=o.view(3, -1, o.shape[1]), n_slots=3, slot_stride=s),
+                    2 * Ms * C * 9 * C, 2 * (Ms * C + 9 * C * C + 2 * 3 * Ms * C))
             if lvl == 0:
-                x2 = torch.randn(B * F, hw, hw, 2 * C, device=dev).half()
+                x2 =torch.randn(B * F, hw, hw, 2 * C, device=dev).half()
                 wc2 = _w(C, 18 * C, dev)
                 cases[f"conv3x3 {M}x{C}x{18 * C}"] = (lambda xi=x2, w=wc2, b=bias, o=out: ops.conv3x3(xi, w, bias=b, out=o),
                                                      2 * M * C * 18 * C, 2 * (M * 2 * C + 18 * C * C + M * C))

@@ -29,11 +29,14 @@ def gemm_pipeline_constants():
 
 
 # ---------------------------------------------------------------------------------------------------------- GEMM ring
-def simulate_gemm_ring(rng: random.Random, nk: int, stages: int, wait_depth: int, dist: int, n_wg: int = 2):
+def simulate_gemm_ring(rng: random.Random, nk: int, stages: int, wait_depth: int, dist: int, n_wg: int = 2,
+                       epilogue_tile: bool = False, tile_shift: int = 0):
     """gemm_wgmma_kernel's K loop.  Per K block kb, every thread: cp.async.wait_group(wait_depth) -> fence -> __syncthreads ->
     issue the loads of block kb + dist into slot (kb + dist) % stages, commit -> wgmma kb on slot kb % stages, commit ->
     wgmma.wait_group(1) (wgmma kb - 1 retired).  Asserts: a block is landed before any wgmma reads it, and a slot is
-    overwritten only after every warpgroup retired the wgmma that read it."""
+    overwritten only after every warpgroup retired the wgmma that read it.  epilogue_tile: after its last wgmma issue a warp
+    starts filling the epilogue's staging tile (cp.async of the residual, or its stores) in slot (nk + tile_shift) % stages
+    without a block barrier: whatever block last held that slot must have been retired by every warpgroup."""
     land = {}
     groups = []  # one cp.async group per prologue stage / iteration, in commit order: the block it loads or None
     retire = [dict() for _ in range(n_wg)]
@@ -61,6 +64,12 @@ def simulate_gemm_ring(rng: random.Random, nk: int, stages: int, wait_depth: int
             issue = T + rng.uniform(0, 3)
             retire[w][kb] = issue + rng.uniform(1, 40)
             t_wg[w] = max(issue, retire[w].get(kb - 1, 0.0))  # wgmma.wait_group(1)
+    if epilogue_tile:
+        slot = (nk + tile_shift) % stages
+        held = [b for b in range(nk) if b % stages == slot]
+        for w in range(n_wg):
+            for v in range(n_wg):
+                assert not held or retire[v][held[-1]] <= t_wg[w], f"staging tile in slot {slot} while block {held[-1]} is still read"
     return True
 
 
@@ -214,11 +223,70 @@ def acc_col(t, i):
     return 8 * (i >> 2) + 2 * (t & 3) + (i & 1)
 
 
+def stage_offset(row, chunk, swizzle=True):
+    """gemm_wgmma.cu stage_offset: byte offset of 16-byte chunk `chunk` of row `row` in the epilogue's staging tile (256-byte rows)"""
+    return row * 256 + ((chunk ^ (row & 7 if swizzle else 0)) << 4)
+
+
+def check_epilogue_staging(geglu: bool, swizzle: bool = True):
+    """The staging tile of gemm_wgmma_kernel's epilogue, per warp (8 warps, warp w holds rows 16 w .. 16 w + 15 of the tile in
+    its accumulators).  (1) Fragment-order 4-byte writes (and the residual reads at the same addresses): one instruction is 8
+    rows x 4 lanes; its 32 lanes hit 32 different banks, and over all instructions every (row, column pair) of the tile is
+    written exactly once.  (2) Copy-out 16-byte reads, lane -> chunk (32 i + lane) of the warp's rows in row-major order: each
+    quarter warp (one shared-memory wavefront of a 128-bit access) covers the 8 bank groups once, the lanes of a row read
+    consecutive chunks (whole 128-byte lines of the output row), and every chunk is read exactly once BY THE WARP THAT WROTE
+    IT — the epilogue orders the two with __syncwarp only.  (3) The residual cp.async pattern (2 rows x 16 chunks per
+    instruction) fetches every chunk once, again in the warp that consumes it.  swizzle=False is the negative control."""
+    src = _src("gemm_wgmma.cu")
+    assert "return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));" in src, "stage_offset changed: update the model"
+    lg = 3 if geglu else 4  # log2(chunks per tile row): the GEGLU output tile is 128 x 64
+    cpr = 1 << lg
+    writer = {}  # byte address of a 4-byte word -> warp
+    for warp in range(8):
+        wg, t0 = warp // 4, (warp % 4) * 32
+        chunks = [4 * g + jj for g in range(2) for jj in range(4)] if geglu else list(range(16))
+        for chunk in chunks:
+            for h in range(2):
+                addrs = [stage_offset(wg * 64 + acc_row(t0 + lane, 0) + 8 * h, chunk, swizzle) + 4 * (lane & 3) for lane in range(32)]
+                assert len({(a // 4) % 32 for a in addrs}) == 32, f"fragment store of chunk {chunk}: bank conflict"
+                for a in addrs:
+                    assert 0 <= a < 128 * 256 and a not in writer, "staging word written twice"
+                    writer[a] = warp
+    want = {stage_offset(r, c, swizzle) + 4 * q for r in range(128) for c in range(cpr) for q in range(4)}
+    assert set(writer) == want, "the fragment stores do not cover the tile"
+    read = set()
+    for warp in range(8):
+        for i in range(8):
+            lanes = [(lane, 16 * warp + ((32 * i + lane) >> lg), (32 * i + lane) & (cpr - 1)) for lane in range(32)
+                     if ((32 * i + lane) >> lg) < 16]
+            for q in range(0, len(lanes), 8):
+                groups = {(stage_offset(r, c, swizzle) // 16) % 8 for _, r, c in lanes[q:q + 8]}
+                assert len(groups) == 8, "copy-out read: bank conflict inside a quarter warp"
+            for (l0, ra, ca), (l1, rb, cb) in zip(lanes, lanes[1:]):
+                assert (rb, cb) == ((ra, ca + 1) if ca + 1 < cpr else (ra + 1, 0)), "copy-out lanes are not consecutive chunks"
+            for _, r, c in lanes:
+                a = stage_offset(r, c, swizzle)
+                assert a not in read and all(writer[a + 4 * q] == warp for q in range(4)), "chunk read twice or by another warp"
+                read.add(a)
+    assert len(read) == 128 * cpr
+    if not geglu:
+        fetched = {}
+        for warp in range(8):
+            for i in range(8):
+                for lane in range(32):
+                    a = stage_offset(16 * warp + 2 * i + (lane >> 4), lane & 15, swizzle)
+                    assert a not in fetched and writer[a] == warp, "residual chunk fetched twice or by another warp"
+                    fetched[a] = warp
+        assert len(fetched) == 128 * 16
+    return True
+
+
 def check_epilogue(geglu_pack, N_geglu=(128, 256, 2560)):
     """gemm_wgmma_kernel's epilogue index arithmetic: (1) the accumulator layout maps the 128 threads x 64 registers of a
     warpgroup one-to-one onto its 64 x 128 block; (2) GEGLU: the (h, gate) columns the kernel pairs (jh, jg = jh + 4 inside
-    each 64-column group, output column n0 / 2 + 32 g + 8 jj + cq) are the pairs geglu_pack interleaved, every output column
-    written once; (3) the up2 phase store maps the low-resolution pixels one-to-one onto the phase's pixels of the output."""
+    each 64-column group; staged at chunk 4 g + jj, element cq of the tile row, i.e. output column n0 / 2 + 32 g + 8 jj + cq)
+    are the pairs geglu_pack interleaved, every output column written once; (3) out_row_offset of an up2 phase maps the
+    low-resolution pixels one-to-one onto the phase's pixels of the output; (4) the staging tile (check_epilogue_staging)."""
     import torch
     seen = {(acc_row(t, i), acc_col(t, i)) for t in range(128) for i in range(64)}
     assert len(seen) == 64 * 128 and all(0 <= r < 64 and 0 <= c < 128 for r, c in seen)
@@ -254,6 +322,8 @@ def check_epilogue(geglu_pack, N_geglu=(128, 256, 2560)):
                 rows.add((n * 2 * H + 2 * i + py) * (2 * W) + 2 * j + px)
             want = {(n * 2 * H + y) * (2 * W) + x for n in range(NF) for y in range(py, 2 * H, 2) for x in range(px, 2 * W, 2)}
             assert rows == want
+    for geglu in (False, True):
+        check_epilogue_staging(geglu)
     return True
 
 
