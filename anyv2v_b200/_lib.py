@@ -67,6 +67,16 @@ class FreeUArgs(Structure):
                 ("Ch", c_int32), ("Cs", c_int32), ("b", c_float), ("s", c_float)]
 
 
+class TileDesc(Structure):
+    _fields_ = [("ptr", c_void_p), ("sc", c_int64), ("sy", c_int64), ("sx", c_int64)]
+
+
+class TileStitchArgs(Structure):
+    _fields_ = [("tiles", c_void_p), ("out", c_void_p), ("on", c_int64), ("oc", c_int64), ("oy", c_int64), ("ox", c_int64),
+                ("N", c_int32), ("C", c_int32), ("H", c_int32), ("W", c_int32), ("tile_rows", c_int32), ("tile_cols", c_int32),
+                ("tile", c_int32), ("step", c_int32), ("blend", c_int32), ("row_limit", c_int32)]
+
+
 #: every symbol include/anyv2v_b200.h declares -> (restype, argtypes)
 EXPORTS = {
     "av2v_abi_version": (c_int, []),
@@ -82,6 +92,7 @@ EXPORTS = {
     "av2v_attn_pnp_f16": (c_int, [POINTER(AttnArgs), c_void_p]),
     "av2v_tattn_fused_f16": (c_int, [POINTER(TAttnFusedArgs), c_void_p]),
     "av2v_freeu_f16": (c_int, [POINTER(FreeUArgs), c_void_p]),
+    "av2v_tile_stitch_f16": (c_int, [POINTER(TileStitchArgs), c_void_p]),
 }
 
 _lib = None

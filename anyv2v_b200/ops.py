@@ -411,6 +411,43 @@ def freeu(hidden, skip, b: float, s: float, out=None):
     return out
 
 
+# ----------------------------------------------------------------------------------------------------------- VAE tiles
+def tile_stitch(tiles, H: int, W: int, tile: int, step: int, blend: int, row_limit: int, out=None):
+    """The seams of diffusers' tiled VAE encode / decode (csrc/vae_tiles.cu): ``tiles[n][i][j]`` is the RAW output [C, t_i, t_j]
+    (any strides) of tile (i, j) of image n, with t_k = min(tile, L - k * step); -> [N, C, H, W] (channels-last unless ``out``
+    is given), the tiles blended as the reference's in-place loop does and their first ``row_limit`` pixels kept."""
+    global _launches
+    N = len(tiles)
+    _require(N > 0 and all(len(r) == len(tiles[0]) for r in tiles) and len(tiles[0]) > 0 and tiles[0][0],
+             "tile_stitch: expected a non-empty [N][rows][cols] table of tiles")
+    rows, cols = len(tiles[0]), len(tiles[0][0])
+    C = tiles[0][0][0].shape[0]
+    dev = tiles[0][0][0].device
+    ext_h = [min(tile, H - i * step) for i in range(rows)]
+    ext_w = [min(tile, W - j * step) for j in range(cols)]
+    table = []
+    for n, image in enumerate(tiles):
+        for i, row in enumerate(image):
+            _require(len(row) == cols, f"tile_stitch: image {n} row {i} has {len(row)} tiles, expected {cols}")
+            for j, t in enumerate(row):
+                _f16_cuda(t, f"tile_stitch.tiles[{n}][{i}][{j}]")
+                _require(t.device == dev and tuple(t.shape) == (C, ext_h[i], ext_w[j]),
+                         f"tile_stitch.tiles[{n}][{i}][{j}]: expected {(C, ext_h[i], ext_w[j])} on {dev}, got {tuple(t.shape)} "
+                         f"on {t.device}")
+                table.append([t.data_ptr(), *t.stride()])
+    if out is None:
+        out = torch.empty(N, H, W, C, device=dev, dtype=torch.float16).permute(0, 3, 1, 2)
+    _f16_cuda(out, "tile_stitch.out")
+    _require(out.device == dev and tuple(out.shape) == (N, C, H, W),
+             f"tile_stitch.out: expected {(N, C, H, W)} on {dev}, got {tuple(out.shape)} on {out.device}")
+    desc = torch.tensor(table, dtype=torch.int64).to(dev)  # [N * rows * cols] av2v_tile_desc
+    a = L.TileStitchArgs(desc.data_ptr(), _p(out), *out.stride(), N, C, H, W, rows, cols, tile, step, blend, row_limit)
+    with _timed(f"tile_stitch N={N} C={C} {H}x{W} tiles={rows}x{cols}"):
+        L.check(L.lib().av2v_tile_stitch_f16(ctypes.byref(a), _stream()), "av2v_tile_stitch_f16")
+    _launches += 1
+    return out
+
+
 # ----------------------------------------------------------------------------------------------------------- attention
 def _reach(t: torch.Tensor, name: str, rows: int, cols: int, offset: int = 0) -> None:
     """a 2-D token matrix must hold columns [0, cols) and reach element offset + (rows - 1) * ld + cols - 1 of its storage"""

@@ -216,6 +216,29 @@ class I2VGenXLPipeline:
         """Disables FreeU if enabled (pipeline_i2vgen_xl.py:646-648)."""
         self.unet.disable_freeu()
 
+    # -- VAE memory knobs (pipeline_i2vgen_xl.py:191-222), forwarded to the VAE ------------------------------------------
+    def _require_vae(self):
+        if self.vae is None:
+            raise ValueError("The pipeline must have `vae` for VAE slicing / tiling: construct it with `vae=`")
+        return self.vae
+
+    def enable_vae_slicing(self):
+        """Encode and decode one frame per VAE pass: the same frames, with the memory of one frame."""
+        self._require_vae().enable_slicing()
+
+    def disable_vae_slicing(self):
+        """Back to one VAE pass for all frames."""
+        self._require_vae().disable_slicing()
+
+    def enable_vae_tiling(self):
+        """Encode and decode frames larger than the VAE's ``tile_sample_min_size`` in overlapping tiles with blended seams
+        (diffusers' tiled VAE): the memory of a VAE pass no longer grows with the frame size."""
+        self._require_vae().enable_tiling()
+
+    def disable_vae_tiling(self):
+        """Back to whole-frame encode and decode."""
+        self._require_vae().disable_tiling()
+
     def register_modules(self, **kwargs):
         for k, v in kwargs.items():
             setattr(self, k, v)

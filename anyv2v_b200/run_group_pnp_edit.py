@@ -196,6 +196,16 @@ def load_checkpoint_into(module: torch.nn.Module, folder: str) -> bool:
     return False
 
 
+def vae_sample_size(folder: str) -> dict:
+    """``{"sample_size": ...}`` from a diffusers-layout ``vae/config.json`` (the tile size of VAE tiling), or {} without one"""
+    path = os.path.join(folder, "config.json")
+    if not os.path.exists(path):
+        return {}
+    with open(path) as f:
+        cfg = json.load(f)
+    return {"sample_size": cfg["sample_size"]} if "sample_size" in cfg else {}
+
+
 def build_pipeline(device, unet_config=None, seed: int = 8888, broadcast: bool = True, with_encoders: bool = False,
                    model_dir: str | None = None, vae_config=None, clip_arch=None):
     """The pipeline of reference :59-66 (``I2VGenXLPipeline.from_pretrained("ali-vilab/i2vgen-xl", fp16)``).  ``model_dir``
@@ -214,10 +224,13 @@ def build_pipeline(device, unet_config=None, seed: int = 8888, broadcast: bool =
     if with_encoders:
         from .encoders import ClipEncoders
         from .vae import SD_VAE_CONFIG as KL_F8_CONFIG, AutoencoderKL
+        vae_kwargs = dict(vae_config or KL_F8_CONFIG)
+        if have_ckpt and "sample_size" not in vae_kwargs:
+            vae_kwargs.update(vae_sample_size(os.path.join(model_dir, "vae")))
         state = torch.random.get_rng_state()
         torch.manual_seed(seed + 7)
         try:
-            vae = AutoencoderKL(**dict(vae_config or KL_F8_CONFIG))
+            vae = AutoencoderKL(**vae_kwargs)
         finally:
             torch.random.set_rng_state(state)
         if have_ckpt:

@@ -239,6 +239,31 @@ typedef struct {
 } av2v_freeu_args;
 int av2v_freeu_f16(const av2v_freeu_args* a, av2v_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * VAE tile stitch: the seam blending of diffusers 0.26.3 `AutoencoderKL.tiled_encode` / `tiled_decode` (enabled through
+ * pipeline_i2vgen_xl.py:207-222 `enable_vae_tiling`) in one pass, from the RAW (unblended) tile outputs.
+ * All lengths are in output pixels.  Along an axis of length L the tiles start every `step` pixels (k = 0 .. ceil(L/step)-1)
+ * and tile k is t_k = min(tile, L - k*step) long; the first `row_limit` pixels of each tile are kept, at k*row_limit.
+ * Seams are blended as the reference's in-place loop does (blend_v, then blend_h, with e = min(t_{k-1}, t_k, blend)):
+ *   b[y] = fp16(fp16(a[t_{k-1} - e + y] * fp32(1 - y/e)) + fp16(b[y] * fp32(y/e)))   for y < e
+ * where the neighbour a is the already blended tile.  Preconditions (checked, AV2V_EINVAL): the kept parts tile [0, L)
+ * exactly and every tile but the last is at least max(row_limit, 2*blend) long — then each output element depends on at
+ * most the four raw tiles (i, j), (i-1, j), (i, j-1), (i-1, j-1) (csrc/vae_tiles.cu).
+ */
+typedef struct {
+  const void* ptr;                      /* tile [C, t_i, t_j] fp16, element (c, y, x) at ptr + c*sc + y*sy + x*sx */
+  int64_t sc, sy, sx;                   /* element strides */
+} av2v_tile_desc;
+typedef struct {
+  const av2v_tile_desc* tiles;          /* DEVICE array [N][tile_rows][tile_cols] */
+  void* out;                            /* [N, C, H, W] fp16, element (n, c, y, x) at out + n*on + c*oc + y*oy + x*ox */
+  int64_t on, oc, oy, ox;               /* element strides of out */
+  int32_t N, C, H, W;
+  int32_t tile_rows, tile_cols;         /* ceil(H / step), ceil(W / step) */
+  int32_t tile, step, blend, row_limit; /* output pixels, the same on both axes */
+} av2v_tile_stitch_args;
+int av2v_tile_stitch_f16(const av2v_tile_stitch_args* a, av2v_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
