@@ -456,34 +456,6 @@ __global__ void __launch_bounds__(kRowsThreads, 1) attn_rows_kernel(const __grid
   });
 }
 
-// 4-D fp16 tensor map over [branches][sequences][tokens][cols] (row stride ld elements, branch stride in elements): a box of
-// 64 columns x box_rows tokens, 128-byte swizzle (the sw128 tile layout), zeros outside the tensor
-int encode_rows_map(CUtensorMap* map, const void* base, int cols, int tokens, int seqs, int branches, int ld,
-                    long long branch_stride, int box_rows) {
-  using Encode = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                              const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                              CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  static Encode encode = nullptr;
-  if (encode == nullptr) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    AV2V_CHECK_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
-    AV2V_REQUIRE(q == cudaDriverEntryPointSuccess && fn != nullptr, AV2V_ECUDA, "attn: cuTensorMapEncodeTiled not available");
-    encode = reinterpret_cast<Encode>(fn);
-  }
-  const cuuint64_t seq_bytes = static_cast<cuuint64_t>(tokens) * ld * 2;
-  const cuuint64_t dims[4] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(tokens), static_cast<cuuint64_t>(seqs),
-                              static_cast<cuuint64_t>(branches)};
-  const cuuint64_t strides[3] = {static_cast<cuuint64_t>(ld) * 2, seq_bytes,
-                                 branches > 1 ? static_cast<cuuint64_t>(branch_stride) * 2 : seq_bytes * seqs};
-  const cuuint32_t box[4] = {HD, static_cast<cuuint32_t>(box_rows), 1, 1}, estr[4] = {1, 1, 1, 1};
-  const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  AV2V_REQUIRE(r == CUDA_SUCCESS, AV2V_ECUDA, "attn: cuTensorMapEncodeTiled failed (%d)", static_cast<int>(r));
-  return AV2V_OK;
-}
-
 // --------------------------------------------------------------------------------------------------- av2v_tattn_fused_f16
 struct TAttnP {
   const __half* x;

@@ -1,12 +1,12 @@
-// wgmma GEMM core of the I2VGen-XL UNet hot path (sm_90a).
+// wgmma GEMM core of the I2VGen-XL UNet hot path (sm_90a): the convolutions.  av2v_gemm_f16 validates every call and sends
+// the LINEAR mode to gemm_linear_ws.cu's persistent kernel; the conv modes run here.
 //
 //   out[slot][m, n] = sum_k A[m, k] * W[n, k] + bias[n] + rowbias[m / rows_per_rowbias, n] + residual[slot][m, n]
 //
 // One CTA computes a 128 x 128 output tile with two warpgroups (rows 0-63 / 64-127), each issuing wgmma.m64n128k16 with
 // both operands in shared memory.  All 256 threads gather the operand tiles with 16-byte cp.async straight from the
 // channels-last activations — the A row of output pixel m for K block kb is the (tap, channel block) the block names, so the
-// 3 x 3 conv (plain, stride 2, one phase of nearest-up x 2), the temporal (3, 1, 1) conv and the two-source skip concat are
-// implicit GEMMs without an im2col buffer; out-of-image taps, ragged rows and the K tail are zero-filled by cp.async.
+// 3 x 3 conv (plain, stride 2, one phase of nearest-up x 2) and the temporal (3, 1, 1) conv are implicit GEMMs without an im2col buffer; out-of-image taps, ragged rows and the K tail are zero-filled by cp.async.
 // kStages = 3 stage ring (32 KB per stage), prefetch distance 1, one wgmma group in flight behind the current one:
 //   top of K block kb: cp.async of block kb landed (wait_group) -> fence.proxy.async -> __syncthreads (also: every warpgroup
 //   retired wgmma kb-2)
@@ -25,11 +25,8 @@
 // will itself consume.  (Issued from inside the K loop, ptxas serializes the wgmma.)  The residual tiles of further slots go
 // to the other two ring slots once every warpgroup has retired its wgmma.  A value is
 // rounded once: the fp32 sum of accumulator and residual is what gets packed, over the residual's place in the tile.  All
-// of a warp's residual reads complete before its first store, so a residual that aliases out stays safe.  GEGLU pairs the
-// h and gate columns (blocks of 32, interleaved by geglu_pack) which the accumulator layout puts in the same thread; its
-// output tile is 128 x 64.
-#include "host_util.cuh"
-#include "ptx.cuh"
+// of a warp's residual reads complete before its first store, so a residual that aliases out stays safe.
+#include "gemm_common.cuh"
 
 namespace av2v {
 namespace {
@@ -40,52 +37,9 @@ constexpr int kThreads = 256;
 constexpr int kTileBytes = BM * BK * 2;  // 16 KB, A and B alike (BM == BN)
 constexpr int kSmemBytes = kStages * 2 * kTileBytes + 1024;
 
-struct GemmP {
-  int mode;
-  const __half* a;
-  const __half* a2;
-  const __half* w;
-  int M, N, K;
-  int lda, lda2, k_split;  // LINEAR (k_split = K for one source)
-  int Hin, Win, chan;      // CONV3X3: input image, channels present (row stride of A)
-  int Ho, Wo, stride;      // CONV3X3: output pixels of the GEMM rows
-  int taps_w, up2, py, px; // CONV3X3: taps per kernel row (3, or 2 for an up2 phase), phase offsets
-  int Cin;                 // CONV3X3 / TCONV3: K per tap
-  int F, HW;               // TCONV3
-  const __half* bias;
-  const __half* rowbias;
-  int rows_per_rowbias;
-  const __half* residual;
-  __half* out;
-  int ldo;
-  int n_slots;
-  long long slot_stride;
-  int geglu;
-  int n_tiles, num_kb;
-};
-
-// Exact-erf GELU, branch-free: gelu(g) = g/2 * erfc(-g/sqrt 2).  With E = erfc(z), z = |g|/sqrt 2:
-//   g < 0: gelu = g/2 * E;   g >= 0: gelu = g - g/2 * E   ->   gelu = max(g, 0) - |g/2| * E.
-// E has the form of the erfcc routine of Numerical Recipes, t = 1 / (1 + z/2), E = t * exp(-z^2 + P(t)), with a degree-5 P
-// fitted in tools/erfc_poly_fit.py: its error is RELATIVE (< 1.4e-5 on z in [0, 5.6], fp32 evaluation included), so the
-// small negative-gate side keeps full fp16 precision.  (An absolute-error erf — A&S 7.1.25, 2.5e-5 — was 20 fp16 ulps off at
-// gates in [-4, -3], where gelu is ~1e-3.)  MUFU rcp + ex2 and ~9 FMAs per element; libdevice erfcf costs more and diverges.
-__device__ __forceinline__ float gelu_erf_fast(float g) {
-  const float z = fabsf(g) * 0.70710678118654752f;
-  float t;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(fmaf(0.5f, z, 1.0f)));
-  float p = fmaf(t, 0.22427836f, -0.69402432f);
-  p = fmaf(p, t, 0.45475456f);
-  p = fmaf(p, t, 0.26681793f);
-  p = fmaf(p, t, 1.01429605f);
-  p = fmaf(p, t, -1.26611602f);
-  const float e = t * ex2_approx(fmaf(-z, z, p) * 1.4426950408889634f);
-  return fmaf(-fabsf(0.5f * g), e, fmaxf(g, 0.0f));
-}
-
 // Per-thread view of the A rows it gathers (rows r0 + 32 i, i = 0..3, of the tile): what the K loop needs to address them.
 struct ARows {
-  long long base[4];  // element offset of the row's pixel (LINEAR: row start; CONV: pixel of tap (0, 0); TCONV: the row)
+  long long base[4];  // element offset of the row's pixel (CONV: pixel of tap (0, 0); TCONV: the row)
   int y[4], x[4];     // CONV: input coordinates of tap (0, 0); TCONV: y = frame; -1 marks a row past M
 };
 
@@ -97,10 +51,7 @@ __device__ __forceinline__ void a_rows_init(const GemmP& p, int m0, int r0, ARow
     ar.x[i] = 0;
     ar.base[i] = 0;
     if (m >= p.M) continue;
-    if (p.mode == AV2V_A_LINEAR) {
-      ar.base[i] = m;
-      ar.y[i] = 0;
-    } else if (p.mode == AV2V_A_CONV3X3) {
+    if (p.mode == AV2V_A_CONV3X3) {
       const int ox = m % p.Wo, t = m / p.Wo, oy = t % p.Ho, n = t / p.Ho;
       const int y0 = p.up2 ? oy - 1 + p.py : oy * p.stride - 1;
       const int x0 = p.up2 ? ox - 1 + p.px : ox * p.stride - 1;
@@ -119,18 +70,7 @@ __device__ __forceinline__ void load_stage(const GemmP& p, const ARows& ar, int 
   const int ch = tid & 7, r0 = tid >> 3;
   const int k0 = kb * BK;
   // ---- A
-  if (p.mode == AV2V_A_LINEAR) {
-    const bool second = k0 >= p.k_split;
-    const __half* src = second ? p.a2 : p.a;
-    const long long ld = second ? p.lda2 : p.lda;
-    const int kk = (second ? k0 - p.k_split : k0) + ch * 8;
-    const bool kval = k0 + ch * 8 < (second ? p.K : p.k_split);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const bool v = kval && ar.y[i] >= 0;
-      cp_async16(sA + sw128_offset(r0 + 32 * i, ch), v ? src + ar.base[i] * ld + kk : p.a, v);
-    }
-  } else if (p.mode == AV2V_A_CONV3X3) {
+  if (p.mode == AV2V_A_CONV3X3) {
     const int tap = k0 / p.Cin, c = k0 - tap * p.Cin + ch * 8;
     const int ky = tap / p.taps_w, kx = tap - ky * p.taps_w;
     const bool cval = c < p.chan;
@@ -247,87 +187,57 @@ __global__ void __launch_bounds__(kThreads, 2) gemm_wgmma_kernel(const __grid_co
     __syncthreads();  // the other ring slots held the last operands: every warpgroup has retired its wgmma
     for (int s = 1; s < n_res; ++s) load_residual_rows(p, s, m0, n0, sA((nk + s) % kStages));
   }
-  if (p.geglu) {
-    const uint32_t tile = sA(nk % kStages);
+  const __half* rb[2];
 #pragma unroll
-    for (int g = 0; g < 2; ++g) {
+  for (int h = 0; h < 2; ++h) {
+    const int m = m0 + r0 + 8 * h;
+    rb[h] = p.rowbias && m < p.M ? p.rowbias + static_cast<long long>(m / p.rows_per_rowbias) * p.N : nullptr;
+  }
+  cp_async_commit();
+  cp_async_wait<0>();
+  __syncwarp();  // the residual chunks this warp's lanes fetched for each other have landed
+  for (int s = 0; s < n_res; ++s) {
+    const uint32_t tile = sA((nk + s) % kStages);
 #pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const int jh = 8 * g + jj, jg = jh + 4;
-        const int ch = n0 + 8 * jh + cq, cg = n0 + 8 * jg + cq;
-        if (ch >= p.N) continue;
-        float2 bh = make_float2(0.f, 0.f), bg = bh;
+    for (int j = 0; j < 16; ++j) {
+      const int c = n0 + 8 * j + cq;
+      if (c >= p.N) continue;
+      float2 b = make_float2(0.f, 0.f);
+      if (p.bias) b = __half22float2(*reinterpret_cast<const __half2*>(p.bias + c));
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t at = tile + stage_offset(r0 + 8 * h, j) + 2 * cq;
+        float o0 = d[4 * j + 2 * h], o1 = d[4 * j + 2 * h + 1];
         if (p.bias) {
-          bh = __half22float2(*reinterpret_cast<const __half2*>(p.bias + ch));
-          bg = __half22float2(*reinterpret_cast<const __half2*>(p.bias + cg));
+          o0 += b.x;
+          o1 += b.y;
         }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          float h0 = d[4 * jh + 2 * h], h1 = d[4 * jh + 2 * h + 1];
-          float g0 = d[4 * jg + 2 * h], g1 = d[4 * jg + 2 * h + 1];
-          if (p.bias) {
-            h0 += bh.x; h1 += bh.y; g0 += bg.x; g1 += bg.y;
-          }
-          st_shared_u32(tile + stage_offset(r0 + 8 * h, 4 * g + jj) + 2 * cq,
-                        pack_half2(h0 * gelu_erf_fast(g0), h1 * gelu_erf_fast(g1)));
+        if (rb[h]) {
+          const float2 t = __half22float2(*reinterpret_cast<const __half2*>(rb[h] + c));
+          o0 += t.x;
+          o1 += t.y;
         }
-      }
-    }
-  } else {
-    const __half* rb[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int m = m0 + r0 + 8 * h;
-      rb[h] = p.rowbias && m < p.M ? p.rowbias + static_cast<long long>(m / p.rows_per_rowbias) * p.N : nullptr;
-    }
-    cp_async_commit();
-    cp_async_wait<0>();
-    __syncwarp();  // the residual chunks this warp's lanes fetched for each other have landed
-    for (int s = 0; s < n_res; ++s) {
-      const uint32_t tile = sA((nk + s) % kStages);
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int c = n0 + 8 * j + cq;
-        if (c >= p.N) continue;
-        float2 b = make_float2(0.f, 0.f);
-        if (p.bias) b = __half22float2(*reinterpret_cast<const __half2*>(p.bias + c));
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const uint32_t at = tile + stage_offset(r0 + 8 * h, j) + 2 * cq;
-          float o0 = d[4 * j + 2 * h], o1 = d[4 * j + 2 * h + 1];
-          if (p.bias) {
-            o0 += b.x;
-            o1 += b.y;
-          }
-          if (rb[h]) {
-            const float2 t = __half22float2(*reinterpret_cast<const __half2*>(rb[h] + c));
-            o0 += t.x;
-            o1 += t.y;
-          }
-          if (p.residual) {
-            const uint32_t rr = ld_shared_u32(at);
-            const float2 r = __half22float2(*reinterpret_cast<const __half2*>(&rr));
-            o0 += r.x;
-            o1 += r.y;
-          }
-          st_shared_u32(at, pack_half2(o0, o1));
+        if (p.residual) {
+          const uint32_t rr = ld_shared_u32(at);
+          const float2 r = __half22float2(*reinterpret_cast<const __half2*>(&rr));
+          o0 += r.x;
+          o1 += r.y;
         }
+        st_shared_u32(at, pack_half2(o0, o1));
       }
     }
   }
   __syncwarp();
 
-  // ---- copy-out: lane -> 16-byte chunk of a row, a warp instruction covers 2 rows x 256 bytes (GEGLU: 4 rows x 128 bytes)
-  const int lg = p.geglu ? 3 : 4;  // log2(chunks per output row of the tile)
-  const int col0 = p.geglu ? n0 / 2 : n0, n_out = p.geglu ? p.N / 2 : p.N;
+  // ---- copy-out: lane -> 16-byte chunk of a row, a warp instruction covers 2 rows x 256 bytes
   for (int s = 0; s < p.n_slots; ++s) {
     const uint32_t tile = sA((nk + (p.residual ? s : 0)) % kStages);
-    __half* out = p.out + s * p.slot_stride + col0;
+    __half* out = p.out + s * p.slot_stride + n0;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int idx = 32 * i + lane;
-      const int r = (threadIdx.x >> 5) * 16 + (idx >> lg), ch = idx & ((1 << lg) - 1);
-      if ((idx >> lg) < 16 && m0 + r < p.M && col0 + 8 * ch < n_out)
+      const int r = (threadIdx.x >> 5) * 16 + (idx >> 4), ch = idx & 15;
+      if (m0 + r < p.M && n0 + 8 * ch < p.N)
         st_global_v4(out + out_row_offset(p, m0 + r) + 8 * ch, ld_shared_v4(tile + stage_offset(r, ch)));
     }
   }
@@ -439,6 +349,7 @@ extern "C" int av2v_gemm_f16(const av2v_gemm_args* a, av2v_stream_t stream_) {
   p.n_tiles = (a->N + BN - 1) / BN;
   const long long tiles = static_cast<long long>((a->M + BM - 1) / BM) * p.n_tiles;
   AV2V_REQUIRE(tiles < (1ll << 31), AV2V_ENOSUP, "gemm: too many tiles");
+  if (p.mode == AV2V_A_LINEAR) return gemm_linear_ws(p, stream);
   static bool attr_set = false;
   if (!attr_set) {
     AV2V_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));

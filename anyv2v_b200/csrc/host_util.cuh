@@ -39,4 +39,8 @@ inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 int sm_count_cached();  // abi.cu
 
+// 4-D fp16 tensor map for TMA tile loads: boxes of 64 columns x box_rows rows, 128-byte swizzle (abi.cu)
+int encode_rows_map(CUtensorMap* map, const void* base, int cols, int tokens, int seqs, int branches, int ld,
+                    long long branch_stride, int box_rows);
+
 }  // namespace av2v

@@ -139,7 +139,7 @@ typedef struct {
   const void* residual;           /* [n_slots][M, N] (ld = ldo) or NULL */
   void* out;                      /* [n_slots][M, ldo] */
   int32_t ldo;                    /* output row stride in elements (>= N, multiple of 8) */
-  int32_t n_slots;                /* >= 1; <= 3 with a residual */
+  int32_t n_slots;                /* >= 1; <= 3 with a residual; 1 in LINEAR mode */
   int64_t slot_stride;            /* elements between slots (residual and out) */
   int32_t geglu;                  /* 1: fused GEGLU epilogue (FeedForward.net[0], SURVEY A.7): w/bias rows are interleaved in
                                      blocks of 32 as [h_0, gate_0, h_1, gate_1, ...]; out has N/2 columns,

@@ -1,4 +1,4 @@
-"""Fit and check the erfc of the GEGLU epilogue (gelu_erf_fast in csrc/gemm_wgmma.cu): erfc(z) = t * exp(-z^2 + P5(t)) with
+"""Fit and check the erfc of the GEGLU epilogue (gelu_erf_fast in csrc/gemm_common.cuh): erfc(z) = t * exp(-z^2 + P5(t)) with
 t = 1 / (1 + z/2) — the form of the erfcc routine of Numerical Recipes, with a degree-5 polynomial fitted here instead of its
 degree-9 one.  The error of this form is RELATIVE, which is what gelu(g) = g/2 * erfc(-g/sqrt 2) needs on the small negative
 side.  Fitted on z in [0, 5.6] (gates down to -7.9; below that |gelu| < 3e-14); emulated in float32 numpy as the device code

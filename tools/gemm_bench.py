@@ -7,7 +7,8 @@ Each round times every shape with CUDA events on this build and then on each oth
 median over rounds of the mean time per call, the achieved TFLOP/s and GB/s (operations and the least HBM bytes of the
 GEMM: A, W, the output and the residual once each), and the share of the shape's bound: max(FLOPs / 989 TFLOP/s,
 bytes / 3.35 TB/s), the H100 SXM data-sheet rates, with the bound named.  The card name, power limit and SM clock are
-printed with the numbers."""
+printed with the numbers.  Before timing, every shape's output is compared with torch.equal against each other build's on
+the same inputs: a change of kernel that keeps the arithmetic must keep every bit."""
 from __future__ import annotations
 
 import argparse
@@ -114,6 +115,13 @@ def main():
         for fn, _, _ in cases.values():
             fn()
     torch.cuda.synchronize()
+    equal = {}
+    for c, (fn, _, _) in cases.items():
+        outs = {}
+        for name, lib in libs.items():
+            _lib._lib = lib
+            outs[name] = fn().clone()
+        equal[c] = all(torch.equal(outs["this"], o) for o in outs.values())
     for _ in range(args.rounds):
         for c, (fn, _, _) in cases.items():
             for name, lib in libs.items():
@@ -126,7 +134,7 @@ def main():
     for c, (_, flops, nbytes) in cases.items():
         bound_us = max(flops / (PEAK_TFLOPS * 1e6), nbytes / (PEAK_GBS * 1e3))
         which = "tensor" if flops / (PEAK_TFLOPS * 1e6) >= nbytes / (PEAK_GBS * 1e3) else "HBM"
-        row = dict(case=c, gflop=round(flops / 1e9, 1), bound=which)
+        row = dict(case=c, gflop=round(flops / 1e9, 1), bound=which, equal=equal[c])
         line = f"{c:32s}"
         for name in libs:
             t = statistics.median(times[(name, c)])
@@ -136,9 +144,14 @@ def main():
                             of_bound=round(bound_us / t, 3))
             line += f" | {tag} {t:9.2f} us {flops / t / 1e6:6.1f} TF/s {nbytes / t / 1e3:7.1f} GB/s {bound_us / t:6.1%} of {which}"
         rows.append(row)
-        print(line)
+        print(line + ("" if equal[c] else " | OUTPUT DIFFERS"))
     print("sum over shapes (one call each):", ", ".join(f"{n if n == 'this' else os.path.basename(os.path.dirname(os.path.abspath(n)))} {t:.1f} us"
                                                    for n, t in total.items()))
+    linear = [c for c in cases if c.split()[0] in ("linear", "linear+res", "linear+rowbias", "geglu")]
+    print("sum over the linear-mode shapes:", ", ".join(f"{n if n == 'this' else os.path.basename(os.path.dirname(os.path.abspath(n)))} "
+                                                        f"{sum(statistics.median(times[(n, c)]) for c in linear):.1f} us" for n in libs))
+    differ = [c for c in cases if not equal[c]]
+    print("outputs torch.equal across builds:", "every shape" if not differ else f"NO, differ on {differ}")
     print(json.dumps(rows))
 
 

@@ -1,4 +1,5 @@
-"""CPU models of the synchronisation and index bookkeeping of the sm_90a kernels (csrc/gemm_wgmma.cu, csrc/attention_wgmma.cu).
+"""CPU models of the synchronisation and index bookkeeping of the sm_90a kernels (csrc/gemm_wgmma.cu, csrc/gemm_linear_ws.cu,
+csrc/attention_wgmma.cu).
 
 A data race or a wrong index in these kernels shows up on the GPU only as occasionally wrong numbers, so the schedules are
 restated here as discrete-event models with randomised latencies and checked for their hazards, each with a negative control
@@ -406,4 +407,126 @@ def simulate_rows_ring(rng: random.Random, n: int, stages: int, arrivals: int = 
             t_wg[w] = retire + rng.uniform(1, 30)  # softmax of tile k
     order = [w for _, w in sorted(turns, key=lambda x: x[0])]
     assert order == [0, 1] * (n + 1), "MMA turns of the two consumers do not alternate"
+    return True
+
+
+# ---------------------------------------------------------------------------------------------------------- persistent LINEAR GEMM
+def linear_ws_constants():
+    """(stages, empty-barrier arrivals) of gemm_linear_ws_kernel's ring, as written in gemm_linear_ws.cu; also checks that the
+    tile schedule, the barrier parities, the turn taking and the staging layout are the ones the models below restate"""
+    s = _src("gemm_linear_ws.cu")
+    stages = int(re.search(r"constexpr int kStages = (\d+);", s).group(1))
+    arrivals = int(re.search(r"mbar_init\(&empty\[s\], (\d+)\);", s).group(1))
+    for rule in ("for (int t = blockIdx.x; t < P.tiles; t += gridDim.x)",
+                 "for (int i = wg, t = blockIdx.x + wg * gridDim.x; t < P.tiles; i += 2, t += 2 * gridDim.x)",
+                 "const int g0 = i * nk;", "const int s = g % kStages, k0 = kb * BK;",
+                 "mbar_wait<false>(&empty[s], ((g / kStages) - 1) & 1)", "mbar_wait<false>(&full[s], (g / kStages) & 1)",
+                 "if (kb > 0) release(g - 1);", "release(g0 + nk - 1);", "if (wg == 1) named_bar_arrive(1, 256);",
+                 "if (t + gridDim.x < P.tiles) hand_over();", "tiles < sm_count_cached() ? tiles : sm_count_cached()",
+                 "return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));"):
+        assert rule in s, f"gemm_linear_ws.cu no longer contains {rule!r}: update the model"
+    return stages, arrivals
+
+
+def linear_ws_schedule(tiles: int, sms: int, off_by_one: bool = False):
+    """the persistent schedule as the kernel walks it: grid = min(tiles, sms) CTAs; per CTA the producer's tile list and
+    each consumer warpgroup's (local index i, tile) list.  Asserts both sides agree, every tile is computed exactly once,
+    and no CTA is idle.  off_by_one: the loops run to t <= tiles (negative control)."""
+    grid = min(tiles, sms)
+    end = tiles + 1 if off_by_one else tiles
+    done = [0] * (tiles + 1)
+    for b in range(grid):
+        prod = list(range(b, end, grid))
+        cons = {wg: list(zip(range(wg, 10 ** 9, 2), range(b + wg * grid, end, 2 * grid))) for wg in (0, 1)}
+        assert prod, f"CTA {b} has no tile"
+        merged = sorted(cons[0] + cons[1])
+        assert [i for i, _ in merged] == list(range(len(prod))) and [t for _, t in merged] == prod, "consumers and producer disagree"
+        for t in prod:
+            assert t < tiles, f"CTA {b} computes tile {t} past the last ({tiles - 1})"
+            done[t] += 1
+    assert all(n == 1 for n in done[:tiles]), "a tile is computed twice or never"
+    return True
+
+
+def simulate_linear_ws(rng: random.Random, n_tiles: int, nk: int, stages: int, arrivals: int = 4, release: bool = True,
+                       wrong_parity: str = "", pingpong: bool = True, early_refill: bool = False):
+    """one CTA of gemm_linear_ws_kernel with n_tiles tiles of nk K blocks.  Producer: block g = i * nk + kb in stage g % S,
+    waits empty with parity ((g / S) - 1) & 1 (g >= S), then TMA (full completes when the bytes land).  Consumer w takes local
+    tiles i = w, w + 2, ...: fetches the tile's residual into its staging tile (cp.async), waits for its turn (warpgroup 1
+    arrives on warpgroup 0's barrier first; a warpgroup hands over after issuing its last MMA when a tile follows), per block
+    waits full with parity (g / S) & 1, issues, and releases block g - 1 once wgmma.wait_group(1) retired it (the last block
+    after wait_group(0)); then the epilogue and the copy-out of the staging tile.  Asserts: no block read before it landed, no
+    stage refilled before its block was released by every consumer warp, the K loops run one at a time in order 0, 1, 0, 1
+    ..., and a staging tile is refilled only after its copy-out read it.  Negative controls: release=False (a warp never
+    arrives on empty), wrong_parity="producer" / "consumer", pingpong=False, early_refill (the next residual fetch issued
+    before the copy-out)."""
+    full = [_MBar(1) for _ in range(stages)]
+    empty = [_MBar(arrivals) for _ in range(stages)]
+    land, released, loops = {}, {}, []
+    t_prod = 0.0
+    t_wg = [rng.uniform(0, 5), rng.uniform(0, 5)]
+    handed = [rng.uniform(0, 1), None]  # handed[w]: when the turn was handed to w (warpgroup 1's opening arrive: tile 0)
+    copy_done = [None, None]      # end of the last copy-out of each staging tile
+    next_fetch = [None, None]     # early_refill: when the next tile's fetch was issued
+    produced = 0
+
+    def produce_until(g_max):
+        nonlocal t_prod, produced
+        while produced <= g_max and produced < n_tiles * nk:
+            g, s = produced, produced % stages
+            if g >= stages:
+                par = ((g // stages) - 1) & 1
+                t_prod = empty[s].wait(par ^ (wrong_parity == "producer"), t_prod)
+                assert released.get(g - stages, float("inf")) <= t_prod, f"stage {s} refilled with block {g} while block {g - stages} is read"
+            t_prod += rng.uniform(0.1, 2)
+            land[g] = t_prod + rng.uniform(5, 60)
+            full[s].arrive(land[g])
+            produced += 1
+
+    def release_block(g, t):
+        n = arrivals if release else arrivals - 1
+        empty[g % stages].arrive(t, n)
+        if release:
+            released[g] = t
+
+    for i in range(n_tiles):
+        w = i % 2
+        t = t_wg[w]
+        fetch = next_fetch[w] if early_refill and next_fetch[w] is not None else t
+        if copy_done[w] is not None:
+            assert copy_done[w] <= fetch, f"staging tile {w} refilled by tile {i} before the copy-out of tile {i - 2} read it"
+        res_land = fetch + rng.uniform(5, 50)
+        if pingpong:
+            assert handed[w] is not None, "a warpgroup waits for a turn nobody hands over (deadlock)"
+            t = max(t, handed[w])
+            handed[w] = None
+        start = t
+        prev_retire = 0.0
+        for kb in range(nk):
+            g = i * nk + kb
+            produce_until(g)
+            t = full[g % stages].wait(((g // stages) & 1) ^ (wrong_parity == "consumer"), t)
+            assert land[g] <= t, f"warpgroup {w} reads block {g} before it landed"
+            t += rng.uniform(0.1, 2)                     # issue
+            retire = t + rng.uniform(5, 30)
+            if kb > 0:
+                t = max(t, prev_retire)                  # wgmma.wait_group(1): block g - 1 retired
+                release_block(g - 1, t)
+            prev_retire = retire
+        loops.append((start, t, w))
+        if i + 1 < n_tiles:
+            handed[1 - w] = t + rng.uniform(0.1, 1)
+        t = max(t, prev_retire)                          # wgmma.wait_group(0)
+        release_block(i * nk + nk - 1, t)
+        t = max(t, res_land) + rng.uniform(5, 40)        # cp.async.wait_group(0), epilogue into the staging tile
+        if early_refill:
+            next_fetch[w] = t
+        t += rng.uniform(5, 40)                          # copy-out
+        copy_done[w] = t
+        t_wg[w] = t
+    produce_until(n_tiles * nk)
+    loops.sort()
+    assert [w for _, _, w in loops] == [i % 2 for i in range(n_tiles)], "the K loops do not take turns 0, 1, 0, 1, ..."
+    for (s0, e0, _), (s1, _, _) in zip(loops, loops[1:]):
+        assert e0 <= s1, "the K loops of the two consumers overlap"
     return True
