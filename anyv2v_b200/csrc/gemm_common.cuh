@@ -1,4 +1,5 @@
-// Shared by the two GEMM kernels: the launch parameters av2v_gemm_f16 validates and fills, and the GEGLU activation.
+// Shared by the two GEMM kernels: the launch parameters av2v_gemm_f16 validates and fills, the GEGLU activation and the
+// staged epilogue.
 //   gemm_wgmma.cu      : the conv modes (3 x 3, stride 2, up2 phase, temporal (3, 1, 1)), two CTAs per SM
 //   gemm_linear_ws.cu  : the LINEAR mode, persistent and warp-specialized
 #pragma once
@@ -50,7 +51,112 @@ __device__ __forceinline__ float gelu_erf_fast(float g) {
   return fmaf(-fabsf(0.5f * g), e, fmaxf(g, 0.0f));
 }
 
-// LINEAR-mode launch (gemm_linear_ws.cu); p is validated and filled by av2v_gemm_f16
-int gemm_linear_ws(const GemmP& p, cudaStream_t stream);
+// ---- staged epilogue.  A 128 x 128 output tile is packed in fp16 into a staging tile in shared memory (128 rows x 256
+// bytes, 16-byte chunk c of row r at chunk c ^ (r & 7): the 8 rows x 4 lanes of a fragment store and the 8 chunks a quarter
+// warp copies out both cover the 32 banks once) and leaves it in 16-byte stores along the output rows.  A warp's unit of
+// work is a band: the 16 tile rows r0 .. r0 + 15 it holds in one m64n128 accumulator (float[64]); a warp with kBands
+// accumulators owns the bands r0 + 64 b.  A warp fetches, writes and copies out only its own bands' rows, so the kernels
+// order these steps with __syncwarp.  N, ldo and slot_stride are multiples of 8, so every chunk is whole: it is stored iff
+// its row < M and its first column < N.  A value is rounded once: acc + bias + rowbias + residual in fp32, packed over the
+// residual's place in the tile.
+__device__ __forceinline__ uint32_t stage_offset(int row, int chunk) {
+  return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));
+}
+
+// The row mapping and the output tile differ by kernel, fixed at compile time so that neither kernel carries the other's:
+// kConv (gemm_wgmma.cu): the rows of an up2 phase are its pixels of the 2x output; otherwise (LINEAR, gemm_linear_ws.cu)
+// row m is out row m and a GEGLU tile is 128 x 64.
+
+// element offset of output row m inside a slot of out / residual
+template <bool kConv>
+__device__ __forceinline__ long long out_row_offset(const GemmP& p, int m) {
+  if (!kConv || !p.up2) return static_cast<long long>(m) * p.ldo;
+  // low-resolution pixel (n, i, j) -> (n, 2 i + py, 2 j + px) of the [NF][2H][2W] output
+  const int j = m % p.Wo, t = m / p.Wo, i = t % p.Ho, n = t / p.Ho;
+  return ((static_cast<long long>(n) * 2 * p.Ho + 2 * i + p.py) * (2 * p.Wo) + 2 * j + p.px) * p.ldo;
+}
+
+// the band at tile rows r0 .. r0 + 15 of the residual tile of `slot` -> staging tile by cp.async: per instruction 2 rows x
+// 16 chunks, zero-filled past M / N
+template <bool kConv>
+__device__ __forceinline__ void fetch_residual_band(const GemmP& p, int slot, int m0, int n0, int r0, uint32_t tile) {
+  const int lane = threadIdx.x & 31, ch = lane & 15;
+  const int c = n0 + 8 * ch;
+  const __half* src = p.residual + slot * p.slot_stride + c;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int r = r0 + 2 * i + (lane >> 4);
+    const bool v = m0 + r < p.M && c < p.N;
+    cp_async16(tile + stage_offset(r, ch), v ? src + out_row_offset<kConv>(p, m0 + r) : p.residual, v);
+  }
+}
+
+// acc + bias + rowbias (+ the residual the tile holds) of the warp's bands -> fp16 pairs in fragment order in the staging
+// tile.  Column pair j is the outer loop, so its bias is loaded once for every band (st.shared clobbers memory).
+template <int kBands>
+__device__ __forceinline__ void epilogue_bands(const GemmP& p, const float (&d)[kBands][64], int m0, int n0, int r0,
+                                               uint32_t tile) {
+  const int fr = r0 + ((threadIdx.x & 31) >> 2);  // the thread's rows fr + 64 b + 8 h (accumulator layout, acc_row)
+  const int cq = 2 * (threadIdx.x & 3);
+  const __half* rb[kBands][2];
+#pragma unroll
+  for (int b = 0; b < kBands; ++b)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = m0 + fr + 64 * b + 8 * h;
+      rb[b][h] = p.rowbias && m < p.M ? p.rowbias + static_cast<long long>(m / p.rows_per_rowbias) * p.N : nullptr;
+    }
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int c = n0 + 8 * j + cq;
+    if (c >= p.N) continue;
+    float2 bias = make_float2(0.f, 0.f);
+    if (p.bias) bias = __half22float2(*reinterpret_cast<const __half2*>(p.bias + c));
+#pragma unroll
+    for (int b = 0; b < kBands; ++b)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t at = tile + stage_offset(fr + 64 * b + 8 * h, j) + 2 * cq;
+        float o0 = d[b][4 * j + 2 * h], o1 = d[b][4 * j + 2 * h + 1];
+        if (p.bias) {
+          o0 += bias.x;
+          o1 += bias.y;
+        }
+        if (rb[b][h]) {
+          const float2 t = __half22float2(*reinterpret_cast<const __half2*>(rb[b][h] + c));
+          o0 += t.x;
+          o1 += t.y;
+        }
+        if (p.residual) {
+          const uint32_t rr = ld_shared_u32(at);
+          const float2 r = __half22float2(*reinterpret_cast<const __half2*>(&rr));
+          o0 += r.x;
+          o1 += r.y;
+        }
+        st_shared_u32(at, pack_half2(o0, o1));
+      }
+  }
+}
+
+// the band at tile rows r0 .. r0 + 15 of the staging tile -> slot `slot` of out: lane -> 16-byte chunk of a row, a warp
+// instruction covers 2 rows x 256 bytes (GEGLU: 4 rows x 128 bytes)
+template <bool kConv>
+__device__ __forceinline__ void copy_out_band(const GemmP& p, int slot, int m0, int n0, int r0, uint32_t tile) {
+  const int lane = threadIdx.x & 31;
+  const bool geglu = !kConv && p.geglu;
+  const int lg = geglu ? 3 : 4;  // log2(chunks per output row of the tile)
+  const int col0 = geglu ? n0 / 2 : n0, n_out = geglu ? p.N / 2 : p.N;
+  __half* out = p.out + slot * p.slot_stride + col0;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int idx = 32 * i + lane;
+    const int r = r0 + (idx >> lg), ch = idx & ((1 << lg) - 1);
+    if ((idx >> lg) < 16 && m0 + r < p.M && col0 + 8 * ch < n_out)
+      st_global_v4(out + out_row_offset<kConv>(p, m0 + r) + 8 * ch, ld_shared_v4(tile + stage_offset(r, ch)));
+  }
+}
+
+// LINEAR-mode launch (gemm_linear_ws.cu) of `tiles` output tiles; p is validated and filled by av2v_gemm_f16
+int gemm_linear_ws(const GemmP& p, int tiles, cudaStream_t stream);
 
 }  // namespace av2v

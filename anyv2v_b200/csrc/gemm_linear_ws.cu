@@ -20,13 +20,12 @@
 // producer refills the stage after the empty phase ((g / kStages) - 1) & 1 has completed (tools/kernel_models.py models
 // this schedule).
 //
-// Epilogue (arithmetic as in gemm_wgmma.cu, so outputs are bit-identical to it): + bias / rowbias in fp32, + residual, one
-// rounding; GEGLU pairs the h and gate columns that geglu_pack interleaves, output tile 128 x 64.  Each consumer warpgroup
-// has its own 32 KB staging tile (128 rows x 256 bytes, 16-byte chunk c of row r at chunk c ^ (r & 7)); each warp owns the
-// 32 rows its accumulators hold (16 of each 64-row half), fetches their residual chunks by cp.async before its K loop,
-// writes the results in fragment order and copies its rows out with 16-byte stores, so a warp needs only __syncwarp: all
-// of a warp's residual reads complete before its first store (a residual that aliases out stays safe), and its copy-out
-// reads complete before the next tile's residual fetch or stores refill the tile.
+// Epilogue: gemm_common.cuh's staged epilogue, shared with gemm_wgmma_kernel; GEGLU pairs the h and gate columns that
+// geglu_pack interleaves, output tile 128 x 64.  Each consumer warpgroup has its own 32 KB staging tile; each warp owns two
+// bands (rows 16 w .. 16 w + 15 and 64 + 16 w .., one per accumulator) and fetches their residual chunks by cp.async
+// before its K loop, so a warp needs only __syncwarp: all of a warp's residual reads complete before its first store (a
+// residual that aliases out stays safe), and its copy-out reads complete before the next tile's residual fetch or stores
+// refill the tile.
 #include "gemm_common.cuh"
 
 namespace av2v {
@@ -46,112 +45,36 @@ struct LinWsP {
   int tiles;
 };
 
-// byte offset of 16-byte chunk `chunk` of row `row` in a staging tile (256-byte rows), the layout of gemm_wgmma.cu's
-__device__ __forceinline__ uint32_t stage_offset(int row, int chunk) {
-  return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));
-}
-
-// this warp's 32 rows (16 per 64-row half) of the residual tile -> staging tile, zero-filled past M / N
-__device__ __forceinline__ void load_residual_rows(const GemmP& p, int m0, int n0, uint32_t tile) {
-  const int lane = threadIdx.x & 31, ch = lane & 15, warp = (threadIdx.x >> 5) & 3;
-  const int c = n0 + 8 * ch;
-  const __half* src = p.residual + c;
-#pragma unroll
-  for (int half = 0; half < 2; ++half)
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int r = 64 * half + 16 * warp + 2 * i + (lane >> 4);
-      const bool v = m0 + r < p.M && c < p.N;
-      cp_async16(tile + stage_offset(r, ch), v ? src + static_cast<long long>(m0 + r) * p.ldo : p.residual, v);
-    }
-}
-
-__device__ __forceinline__ void epilogue(const GemmP& p, float (&d)[2][64], int m0, int n0, uint32_t tile) {
+// GEGLU: h * gelu(gate) of the accumulator column pairs jh = 8 g + jj and jg = jh + 4 (the pairs geglu_pack interleaves)
+// -> chunk 4 g + jj of the 128 x 64 output tile, for the rows of both bands
+__device__ __forceinline__ void geglu_epilogue(const GemmP& p, float (&d)[2][64], int n0, uint32_t tile) {
   const int cq = 2 * (threadIdx.x & 3);
-  if (p.geglu) {
 #pragma unroll
-    for (int g = 0; g < 2; ++g) {
+  for (int g = 0; g < 2; ++g) {
 #pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const int jh = 8 * g + jj, jg = jh + 4;
-        const int ch = n0 + 8 * jh + cq, cg = n0 + 8 * jg + cq;
-        if (ch >= p.N) continue;
-        float2 bh = make_float2(0.f, 0.f), bg = bh;
-        if (p.bias) {
-          bh = __half22float2(*reinterpret_cast<const __half2*>(p.bias + ch));
-          bg = __half22float2(*reinterpret_cast<const __half2*>(p.bias + cg));
-        }
+    for (int jj = 0; jj < 4; ++jj) {
+      const int jh = 8 * g + jj, jg = jh + 4;
+      const int ch = n0 + 8 * jh + cq, cg = n0 + 8 * jg + cq;
+      if (ch >= p.N) continue;
+      float2 bh = make_float2(0.f, 0.f), bg = bh;
+      if (p.bias) {
+        bh = __half22float2(*reinterpret_cast<const __half2*>(p.bias + ch));
+        bg = __half22float2(*reinterpret_cast<const __half2*>(p.bias + cg));
+      }
 #pragma unroll
-        for (int half = 0; half < 2; ++half)
+      for (int half = 0; half < 2; ++half)
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            float h0 = d[half][4 * jh + 2 * h], h1 = d[half][4 * jh + 2 * h + 1];
-            float g0 = d[half][4 * jg + 2 * h], g1 = d[half][4 * jg + 2 * h + 1];
-            if (p.bias) {
-              h0 += bh.x; h1 += bh.y; g0 += bg.x; g1 += bg.y;
-            }
-            st_shared_u32(tile + stage_offset(64 * half + acc_row(0) + 8 * h, 4 * g + jj) + 2 * cq,
-                          pack_half2(h0 * gelu_erf_fast(g0), h1 * gelu_erf_fast(g1)));
+        for (int h = 0; h < 2; ++h) {
+          float h0 = d[half][4 * jh + 2 * h], h1 = d[half][4 * jh + 2 * h + 1];
+          float g0 = d[half][4 * jg + 2 * h], g1 = d[half][4 * jg + 2 * h + 1];
+          if (p.bias) {
+            h0 += bh.x; h1 += bh.y; g0 += bg.x; g1 += bg.y;
           }
-      }
+          st_shared_u32(tile + stage_offset(64 * half + acc_row(0) + 8 * h, 4 * g + jj) + 2 * cq,
+                        pack_half2(h0 * gelu_erf_fast(g0), h1 * gelu_erf_fast(g1)));
+        }
     }
-    return;
   }
-  const __half* rb[2][2];
-#pragma unroll
-  for (int half = 0; half < 2; ++half)
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int m = m0 + 64 * half + acc_row(0) + 8 * h;
-      rb[half][h] = p.rowbias && m < p.M ? p.rowbias + static_cast<long long>(m / p.rows_per_rowbias) * p.N : nullptr;
-    }
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    const int c = n0 + 8 * j + cq;
-    if (c >= p.N) continue;
-    float2 b = make_float2(0.f, 0.f);
-    if (p.bias) b = __half22float2(*reinterpret_cast<const __half2*>(p.bias + c));
-#pragma unroll
-    for (int half = 0; half < 2; ++half)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const uint32_t at = tile + stage_offset(64 * half + acc_row(0) + 8 * h, j) + 2 * cq;
-        float o0 = d[half][4 * j + 2 * h], o1 = d[half][4 * j + 2 * h + 1];
-        if (p.bias) {
-          o0 += b.x;
-          o1 += b.y;
-        }
-        if (rb[half][h]) {
-          const float2 t = __half22float2(*reinterpret_cast<const __half2*>(rb[half][h] + c));
-          o0 += t.x;
-          o1 += t.y;
-        }
-        if (p.residual) {
-          const uint32_t rr = ld_shared_u32(at);
-          const float2 r = __half22float2(*reinterpret_cast<const __half2*>(&rr));
-          o0 += r.x;
-          o1 += r.y;
-        }
-        st_shared_u32(at, pack_half2(o0, o1));
-      }
-  }
-}
-
-// lane -> 16-byte chunk of a row, a warp instruction covers 2 rows x 256 bytes (GEGLU: 4 rows x 128 bytes)
-__device__ __forceinline__ void copy_out(const GemmP& p, int m0, int n0, uint32_t tile) {
-  const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
-  const int lg = p.geglu ? 3 : 4;  // log2(chunks per output row of the tile)
-  const int col0 = p.geglu ? n0 / 2 : n0, n_out = p.geglu ? p.N / 2 : p.N;
-  __half* out = p.out + col0;
-#pragma unroll
-  for (int half = 0; half < 2; ++half)
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int idx = 32 * i + lane;
-      const int r = 64 * half + 16 * warp + (idx >> lg), ch = idx & ((1 << lg) - 1);
-      if ((idx >> lg) < 16 && m0 + r < p.M && col0 + 8 * ch < n_out)
-        st_global_v4(out + static_cast<long long>(m0 + r) * p.ldo + 8 * ch, ld_shared_v4(tile + stage_offset(r, ch)));
-    }
 }
 
 __global__ void __launch_bounds__(kThreads, 1) gemm_linear_ws_kernel(const __grid_constant__ LinWsP P) {
@@ -207,10 +130,13 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_linear_ws_kernel(const __gri
   };
   if (wg == 1) named_bar_arrive(1, 256);
 
+  const int r0 = 16 * ((threadIdx.x >> 5) & 3);  // the warp's bands: tile rows r0 .. r0 + 15 and r0 + 64 ..
   float d[2][64];
   for (int i = wg, t = blockIdx.x + wg * gridDim.x; t < P.tiles; i += 2, t += 2 * gridDim.x) {
     const int m0 = t / p.n_tiles * BM, n0 = t % p.n_tiles * BN;
-    if (p.residual) load_residual_rows(p, m0, n0, staging);
+    if (p.residual)
+#pragma unroll
+      for (int b = 0; b < 2; ++b) fetch_residual_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);
     cp_async_commit();
 #pragma unroll
     for (int h = 0; h < 2; ++h)
@@ -242,17 +168,18 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_linear_ws_kernel(const __gri
 
     cp_async_wait<0>();
     __syncwarp();  // the residual chunks this warp's lanes fetched for each other have landed
-    epilogue(p, d, m0, n0, staging);
+    if (p.geglu) geglu_epilogue(p, d, n0, staging);
+    else epilogue_bands<2>(p, d, m0, n0, r0, staging);
     __syncwarp();
-    copy_out(p, m0, n0, staging);
+#pragma unroll
+    for (int b = 0; b < 2; ++b) copy_out_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);
     __syncwarp();  // every lane's copy-out reads are done before the next tile refills the warp's rows
   }
 }
 
 }  // namespace
 
-int gemm_linear_ws(const GemmP& g, cudaStream_t stream) {
-  AV2V_REQUIRE(g.n_slots == 1, AV2V_ENOSUP, "gemm/linear: one output slot only (got n_slots = %d)", g.n_slots);
+int gemm_linear_ws(const GemmP& g, int tiles, cudaStream_t stream) {
   LinWsP P{};
   P.g = g;
   if (int e = encode_rows_map(&P.ta, g.a, g.k_split, g.M, 1, 1, g.lda, 0, BM)) return e;
@@ -260,8 +187,7 @@ int gemm_linear_ws(const GemmP& g, cudaStream_t stream) {
   if (g.a2 != nullptr)
     if (int e = encode_rows_map(&P.ta2, g.a2, g.K - g.k_split, g.M, 1, 1, g.lda2, 0, BM)) return e;
   if (int e = encode_rows_map(&P.tw, g.w, g.K, g.N, 1, 1, g.K, 0, BN)) return e;
-  const long long tiles = static_cast<long long>((g.M + BM - 1) / BM) * g.n_tiles;
-  P.tiles = static_cast<int>(tiles);
+  P.tiles = tiles;
   static bool attr_set = false;
   if (!attr_set) {
     AV2V_CHECK_CUDA(cudaFuncSetAttribute(gemm_linear_ws_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));

@@ -14,18 +14,12 @@
 // Two CTAs per SM (2 x 97 KB of shared memory, <= 128 registers per thread): one CTA's prologue loads, K-loop gathers and
 // epilogue run while the other's wgmma keep the tensor cores busy.  A tile's K loop is short (5 blocks at K = 320), so
 // this overlap between tiles is worth more than a deeper ring inside one: with 4 stages only one CTA fits.
-// Epilogue through shared memory, each warp on its own 16 rows of the tile (the rows its accumulators hold), so it needs no
-// block barrier: + bias / rowbias in the registers, then per slot + residual, fp16 pairs written in accumulator order to a
-// 128 x 128 staging tile (256-byte rows, 16-byte chunk c of row r at chunk c ^ (r & 7): the 8 rows x 4 lanes of a fragment
-// store and the 8 chunks a quarter warp copies out both cover the 32 banks once), __syncwarp, and the warp copies its rows
-// out with 16-byte stores, consecutive lanes on consecutive chunks of one output row (whole 128-byte lines; N, ldo and
-// slot_stride are multiples of 8, so every chunk is whole: stored iff its row < M and its first column < N).  The tile
-// takes the ring slot that block num_kb - 3 left, free from the top of the last K block, and the residual tile of slot 0 is
-// fetched there by cp.async as soon as the last wgmma are issued, so it lands under them; each warp fetches the chunks it
-// will itself consume.  (Issued from inside the K loop, ptxas serializes the wgmma.)  The residual tiles of further slots go
-// to the other two ring slots once every warpgroup has retired its wgmma.  A value is
-// rounded once: the fp32 sum of accumulator and residual is what gets packed, over the residual's place in the tile.  All
-// of a warp's residual reads complete before its first store, so a residual that aliases out stays safe.
+// Epilogue: gemm_common.cuh's staged epilogue, each warp on one band (the 16 tile rows its accumulators hold), so it needs
+// no block barrier.  The staging tile of slot 0 takes the ring slot that block num_kb - 3 left, free from the top of the
+// last K block, and the residual tile of slot 0 is fetched there by cp.async as soon as the last wgmma are issued, so it
+// lands under them.  (Issued from inside the K loop, ptxas serializes the wgmma.)  The residual tiles of further slots go
+// to the other two ring slots once every warpgroup has retired its wgmma.  All of a warp's residual reads complete before
+// its first store, so a residual that aliases out stays safe.
 #include "gemm_common.cuh"
 
 namespace av2v {
@@ -101,32 +95,6 @@ __device__ __forceinline__ void load_stage(const GemmP& p, const ARows& ar, int 
   }
 }
 
-// ---- epilogue staging tile: one ring slot (2 * kTileBytes = 128 rows x 256 bytes), XOR-swizzled like the operand tiles
-__device__ __forceinline__ uint32_t stage_offset(int row, int chunk) {
-  return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));
-}
-
-// element offset of output row m inside a slot of out / residual
-__device__ __forceinline__ long long out_row_offset(const GemmP& p, int m) {
-  if (!p.up2) return static_cast<long long>(m) * p.ldo;
-  // low-resolution pixel (n, i, j) -> (n, 2 i + py, 2 j + px) of the [NF][2H][2W] output
-  const int j = m % p.Wo, t = m / p.Wo, i = t % p.Ho, n = t / p.Ho;
-  return ((static_cast<long long>(n) * 2 * p.Ho + 2 * i + p.py) * (2 * p.Wo) + 2 * j + p.px) * p.ldo;
-}
-
-// This warp's 16 rows of the residual tile of `slot` -> staging tile: per instruction 2 rows x 16 chunks, zero-filled past M / N
-__device__ __forceinline__ void load_residual_rows(const GemmP& p, int slot, int m0, int n0, uint32_t tile) {
-  const int lane = threadIdx.x & 31, ch = lane & 15;
-  const int c = n0 + 8 * ch;
-  const __half* src = p.residual + slot * p.slot_stride + c;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int r = (threadIdx.x >> 5) * 16 + 2 * i + (lane >> 4);
-    const bool v = m0 + r < p.M && c < p.N;
-    cp_async16(tile + stage_offset(r, ch), v ? src + out_row_offset(p, m0 + r) : p.residual, v);
-  }
-}
-
 __global__ void __launch_bounds__(kThreads, 2) gemm_wgmma_kernel(const __grid_constant__ GemmP p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -142,9 +110,9 @@ __global__ void __launch_bounds__(kThreads, 2) gemm_wgmma_kernel(const __grid_co
   ARows ar;
   a_rows_init(p, m0, threadIdx.x >> 3, ar);
 
-  float d[64];
+  float d[1][64];  // the warp's band: tile rows 16 * warp .. + 15
 #pragma unroll
-  for (int i = 0; i < 64; ++i) d[i] = 0.f;
+  for (int i = 0; i < 64; ++i) d[0][i] = 0.f;
 
   const int nk = p.num_kb;
 #pragma unroll
@@ -167,80 +135,29 @@ __global__ void __launch_bounds__(kThreads, 2) gemm_wgmma_kernel(const __grid_co
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < BK / 16; ++k)
-      wgmma_m64n128_ss(d, sw128_desc(a_base + k * 32), sw128_desc(b_base + k * 32), 1);
+      wgmma_m64n128_ss(d[0], sw128_desc(a_base + k * 32), sw128_desc(b_base + k * 32), 1);
     wgmma_commit();
     wgmma_wait<1>();
-    reg_fence(d);
+    reg_fence(d[0]);
   }
   // the ring slot block nk - 3 left stays free: the residual tile of slot 0 is fetched there under the last wgmma
-  if (p.residual) load_residual_rows(p, 0, m0, n0, sA(nk % kStages));
+  const int r0 = 16 * (threadIdx.x >> 5);
+  if (p.residual) fetch_residual_band<true>(p, 0, m0, n0, r0, sA(nk % kStages));
   wgmma_wait<0>();
-  reg_fence(d);
+  reg_fence(d[0]);
 
-  // ---- epilogue: thread owns rows r, r + 8 and column pairs 8 j + 2 (lane & 3) of its warp's 16 rows; staging tile of
-  // slot s = ring slot (nk + s) % kStages
-  const int lane = threadIdx.x & 31;
-  const int r0 = wg * 64 + acc_row(0);
-  const int cq = 2 * (threadIdx.x & 3);
+  // ---- epilogue: the staging tile of slot s is ring slot (nk + s) % kStages
   const int n_res = p.residual ? p.n_slots : 1;  // distinct tiles: without a residual every slot stores the same one
   if (n_res > 1) {
     __syncthreads();  // the other ring slots held the last operands: every warpgroup has retired its wgmma
-    for (int s = 1; s < n_res; ++s) load_residual_rows(p, s, m0, n0, sA((nk + s) % kStages));
-  }
-  const __half* rb[2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int m = m0 + r0 + 8 * h;
-    rb[h] = p.rowbias && m < p.M ? p.rowbias + static_cast<long long>(m / p.rows_per_rowbias) * p.N : nullptr;
+    for (int s = 1; s < n_res; ++s) fetch_residual_band<true>(p, s, m0, n0, r0, sA((nk + s) % kStages));
   }
   cp_async_commit();
   cp_async_wait<0>();
   __syncwarp();  // the residual chunks this warp's lanes fetched for each other have landed
-  for (int s = 0; s < n_res; ++s) {
-    const uint32_t tile = sA((nk + s) % kStages);
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int c = n0 + 8 * j + cq;
-      if (c >= p.N) continue;
-      float2 b = make_float2(0.f, 0.f);
-      if (p.bias) b = __half22float2(*reinterpret_cast<const __half2*>(p.bias + c));
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const uint32_t at = tile + stage_offset(r0 + 8 * h, j) + 2 * cq;
-        float o0 = d[4 * j + 2 * h], o1 = d[4 * j + 2 * h + 1];
-        if (p.bias) {
-          o0 += b.x;
-          o1 += b.y;
-        }
-        if (rb[h]) {
-          const float2 t = __half22float2(*reinterpret_cast<const __half2*>(rb[h] + c));
-          o0 += t.x;
-          o1 += t.y;
-        }
-        if (p.residual) {
-          const uint32_t rr = ld_shared_u32(at);
-          const float2 r = __half22float2(*reinterpret_cast<const __half2*>(&rr));
-          o0 += r.x;
-          o1 += r.y;
-        }
-        st_shared_u32(at, pack_half2(o0, o1));
-      }
-    }
-  }
+  for (int s = 0; s < n_res; ++s) epilogue_bands<1>(p, d, m0, n0, r0, sA((nk + s) % kStages));
   __syncwarp();
-
-  // ---- copy-out: lane -> 16-byte chunk of a row, a warp instruction covers 2 rows x 256 bytes
-  for (int s = 0; s < p.n_slots; ++s) {
-    const uint32_t tile = sA((nk + (p.residual ? s : 0)) % kStages);
-    __half* out = p.out + s * p.slot_stride + n0;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int idx = 32 * i + lane;
-      const int r = (threadIdx.x >> 5) * 16 + (idx >> 4), ch = idx & 15;
-      if (m0 + r < p.M && n0 + 8 * ch < p.N)
-        st_global_v4(out + out_row_offset(p, m0 + r) + 8 * ch, ld_shared_v4(tile + stage_offset(r, ch)));
-    }
-  }
+  for (int s = 0; s < p.n_slots; ++s) copy_out_band<true>(p, s, m0, n0, r0, sA((nk + (p.residual ? s : 0)) % kStages));
 }
 
 }  // namespace
@@ -305,6 +222,7 @@ extern "C" int av2v_gemm_f16(const av2v_gemm_args* a, av2v_stream_t stream_) {
       p.lda2 = a->lda2;
       p.k_split = a->k_split;
     }
+    AV2V_REQUIRE(a->n_slots == 1, AV2V_ENOSUP, "gemm/linear: one output slot only (got n_slots = %d)", a->n_slots);
   } else if (a->mode == AV2V_A_CONV3X3) {
     AV2V_REQUIRE(a->NF > 0 && a->H > 0 && a->W > 0 && a->Cin > 0, AV2V_EINVAL, "gemm/conv3x3: bad geometry");
     AV2V_REQUIRE(a->Cin % BK == 0, AV2V_ENOSUP, "gemm/conv3x3: Cin must be a multiple of 64 (got %d)", a->Cin);
@@ -349,7 +267,7 @@ extern "C" int av2v_gemm_f16(const av2v_gemm_args* a, av2v_stream_t stream_) {
   p.n_tiles = (a->N + BN - 1) / BN;
   const long long tiles = static_cast<long long>((a->M + BM - 1) / BM) * p.n_tiles;
   AV2V_REQUIRE(tiles < (1ll << 31), AV2V_ENOSUP, "gemm: too many tiles");
-  if (p.mode == AV2V_A_LINEAR) return gemm_linear_ws(p, stream);
+  if (p.mode == AV2V_A_LINEAR) return gemm_linear_ws(p, static_cast<int>(tiles), stream);
   static bool attr_set = false;
   if (!attr_set) {
     AV2V_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));

@@ -25,7 +25,7 @@ Why these numbers:
       across one spacing leaves O(2^-11)); a directed rounding moves one of the two statistics by 1/2, so BETA is an eighth
       of the smallest store defect the check is for.  What correct arithmetic can leave in the mean: fp32 operations round to
       nearest (no bias); an approximation with a one-sided relative error r moves a result by at most r |ref| / ulp16(ref) <
-      r 2^11 ulp16.  The largest such r any kernel applies to its result is the GEGLU erfc fit, 1.4e-5 (csrc/gemm_wgmma.cu,
+      r 2^11 ulp16.  The largest such r any kernel applies to its result is the GEGLU erfc fit, 1.4e-5 (csrc/gemm_common.cuh,
       tools/erfc_poly_fit.py): 0.029 ulp16, half of BETA.  ex2.approx and rcp.approx (GroupNorm's SiLU, the erfc's t) stay
       below 2^-22: 2^-11 ulp16.  Attention needs no β of its own: P is rounded to fp16 by round-to-nearest (no bias), and the
       relative error of ex2_poly (7.5e-5, csrc/ptx.cuh) is a factor on each weight that the normalisation divides out where V

@@ -1,4 +1,4 @@
-"""CPU test of the model of gemm_wgmma_kernel's staged epilogue (tools/kernel_models.py: check_epilogue_staging)."""
+"""CPU test of the model of the GEMM kernels' shared staged epilogue (tools/kernel_models.py: check_epilogue_staging)."""
 import os
 import sys
 
@@ -8,14 +8,15 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
-@pytest.mark.parametrize("geglu", [False, True])
-def test_staging_tile_layout(geglu):
-    """every (row, column pair) of the tile is written by one thread and read by one 16-byte copy-out lane of the same warp,
-    both patterns free of bank conflicts per shared-memory wavefront; without the XOR swizzle the fragment stores conflict"""
+@pytest.mark.parametrize("kernel,geglu", [("conv", False), ("linear", False), ("linear", True)])
+def test_staging_tile_layout(kernel, geglu):
+    """for the band ownership of each kernel (conv: 8 warps x 1 band, linear: 4 warps x 2 bands per staging tile), every
+    (row, column pair) of the tile is written by one thread and read by one 16-byte copy-out lane of the same warp, both
+    patterns free of bank conflicts per shared-memory wavefront; without the XOR swizzle the fragment stores conflict"""
     from tools import kernel_models as km
-    assert km.check_epilogue_staging(geglu)
+    assert km.check_epilogue_staging(kernel, geglu)
     with pytest.raises(AssertionError, match="fragment store .* bank conflict"):
-        km.check_epilogue_staging(geglu, swizzle=False)
+        km.check_epilogue_staging(kernel, geglu, swizzle=False)
 
 
 def test_residual_tile_takes_a_free_ring_slot():

@@ -1,6 +1,7 @@
-"""GPU tests of the GEMM's staged epilogue (csrc/gemm_wgmma.cu): the output tile leaves shared memory in 16-byte chunks, so the
-cases here are the ones where a chunk could be written that should not be — a row stride wider than N (the gap must keep its
-poison), N of one chunk and N with a single chunk past a 64-column boundary, and a 3-slot residual that aliases the output.
+"""GPU tests of the staged epilogue both GEMM kernels share (csrc/gemm_common.cuh): the output tile leaves shared memory
+in 16-byte chunks, so the cases here are the ones where a chunk could be written that should not be — a row stride wider
+than N (the gap must keep its poison), N of one chunk and N with a single chunk past a 64-column boundary (LINEAR, GEGLU),
+and a 3-slot residual that aliases the output (conv).
 Float64 contracts of tests/kernel_contracts.py within ulp16(ref) + kappa * cond, on guarded buffers (tests/guarded.py)."""
 import pytest
 import torch

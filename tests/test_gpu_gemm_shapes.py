@@ -1,5 +1,6 @@
-"""GPU tests of the GEMM (csrc/gemm_wgmma.cu) against the float64 contracts of tests/kernel_contracts.py, within
-ulp16(ref) + kappa * cond (tests/ulp_check.py), on guarded buffers (tests/guarded.py).
+"""GPU tests of the GEMM (csrc/gemm_wgmma.cu: the conv modes, csrc/gemm_linear_ws.cu: LINEAR) against the float64
+contracts of tests/kernel_contracts.py, within ulp16(ref) + kappa * cond (tests/ulp_check.py), on guarded buffers
+(tests/guarded.py).
 
 Every A mode and epilogue at full and ragged column tiles (N = 320, 384, 136, 256), shapes with many more tiles than the
 resident CTAs, K loops shorter and longer than the stage ring (K = 64, 320, 1280), ragged M, and the step's full-size

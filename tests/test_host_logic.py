@@ -348,7 +348,8 @@ def test_lean_gemm_epilogue_bookkeeping_model():
     """gemm_wgmma_kernel: (1) the cp.async stage ring with the stage count, wait_group depth and prefetch distance read from
     csrc/gemm_wgmma.cu — every block lands before a wgmma reads it and no slot is refilled before both warpgroups retired the
     wgmma that read it, under randomised latencies; a prefetch one block further or a laxer wait_group is caught; (2) the
-    register epilogue's index arithmetic: accumulator layout, GEGLU (h, gate) pairing against geglu_pack, up2 phase rows."""
+    GEMM epilogues' index arithmetic: accumulator layout, GEGLU (h, gate) pairing against geglu_pack, up2 phase rows, and
+    the staging tile of each kernel's band ownership."""
     import random
     from tools import kernel_models as km
     sys.path.insert(0, os.path.join(ROOT, "tests"))

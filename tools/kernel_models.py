@@ -1,5 +1,5 @@
 """CPU models of the synchronisation and index bookkeeping of the sm_90a kernels (csrc/gemm_wgmma.cu, csrc/gemm_linear_ws.cu,
-csrc/attention_wgmma.cu).
+csrc/gemm_common.cuh, csrc/attention_wgmma.cu).
 
 A data race or a wrong index in these kernels shows up on the GPU only as occasionally wrong numbers, so the schedules are
 restated here as discrete-event models with randomised latencies and checked for their hazards, each with a negative control
@@ -225,69 +225,90 @@ def acc_col(t, i):
 
 
 def stage_offset(row, chunk, swizzle=True):
-    """gemm_wgmma.cu stage_offset: byte offset of 16-byte chunk `chunk` of row `row` in the epilogue's staging tile (256-byte rows)"""
+    """gemm_common.cuh stage_offset: byte offset of 16-byte chunk `chunk` of row `row` in the epilogue's staging tile (256-byte rows)"""
     return row * 256 + ((chunk ^ (row & 7 if swizzle else 0)) << 4)
 
 
-def check_epilogue_staging(geglu: bool, swizzle: bool = True):
-    """The staging tile of gemm_wgmma_kernel's epilogue, per warp (8 warps, warp w holds rows 16 w .. 16 w + 15 of the tile in
-    its accumulators).  (1) Fragment-order 4-byte writes (and the residual reads at the same addresses): one instruction is 8
-    rows x 4 lanes; its 32 lanes hit 32 different banks, and over all instructions every (row, column pair) of the tile is
-    written exactly once.  (2) Copy-out 16-byte reads, lane -> chunk (32 i + lane) of the warp's rows in row-major order: each
-    quarter warp (one shared-memory wavefront of a 128-bit access) covers the 8 bank groups once, the lanes of a row read
-    consecutive chunks (whole 128-byte lines of the output row), and every chunk is read exactly once BY THE WARP THAT WROTE
-    IT — the epilogue orders the two with __syncwarp only.  (3) The residual cp.async pattern (2 rows x 16 chunks per
-    instruction) fetches every chunk once, again in the warp that consumes it.  swizzle=False is the negative control."""
-    src = _src("gemm_wgmma.cu")
+def epilogue_bands(kernel: str):
+    """warp -> first tile rows of the bands it owns in one staging tile: the rows its accumulators hold (acc_row).
+    conv (gemm_wgmma_kernel): 8 warps, warpgroup wg's one accumulator holds tile rows 64 wg .. 64 wg + 63.
+    linear (gemm_linear_ws_kernel): a consumer warpgroup's own tile, 4 warps, accumulator b holds tile rows 64 b .. 64 b + 63."""
+    if kernel == "conv":
+        return {w: [64 * (w // 4) + acc_row(32 * (w % 4), 0)] for w in range(8)}
+    assert kernel == "linear", kernel
+    return {w: [64 * b + acc_row(32 * w, 0) for b in range(2)] for w in range(4)}
+
+
+def check_epilogue_staging(kernel: str, geglu: bool = False, swizzle: bool = True):
+    """The staging tile of the GEMM epilogue (gemm_common.cuh), per warp and band (epilogue_bands: a band is the 16 rows a
+    warp holds in one accumulator; conv: 8 warps x 1 band, linear: 4 warps x 2 bands, GEGLU in linear only).  (1)
+    Fragment-order 4-byte writes (and the residual reads at the same addresses): one instruction is 8 rows x 4 lanes; its 32
+    lanes hit 32 different banks, and over all instructions every (row, column pair) of the tile is written exactly once.
+    (2) Copy-out 16-byte reads, lane -> chunk (32 i + lane) of the band's rows in row-major order: each quarter warp (one
+    shared-memory wavefront of a 128-bit access) covers the 8 bank groups once, the lanes of a row read consecutive chunks
+    (whole 128-byte lines of the output row), and every chunk is read exactly once BY THE WARP THAT WROTE IT — the kernels
+    order the two with __syncwarp only.  (3) The residual cp.async pattern (2 rows x 16 chunks per instruction) fetches
+    every chunk once, again in the warp that consumes it.  swizzle=False is the negative control."""
+    assert not (geglu and kernel == "conv"), "GEGLU runs on gemm_linear_ws_kernel only"
+    src = _src("gemm_common.cuh")
     assert "return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));" in src, "stage_offset changed: update the model"
+    for f, rule in (("gemm_wgmma.cu", "const int r0 = 16 * (threadIdx.x >> 5);"),
+                    ("gemm_linear_ws.cu", "const int r0 = 16 * ((threadIdx.x >> 5) & 3);"),
+                    ("gemm_linear_ws.cu", "fetch_residual_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);"),
+                    ("gemm_linear_ws.cu", "copy_out_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);")):
+        assert rule in _src(f), f"{f} no longer contains {rule!r}: update the model"
+    bands = epilogue_bands(kernel)
     lg = 3 if geglu else 4  # log2(chunks per tile row): the GEGLU output tile is 128 x 64
     cpr = 1 << lg
     writer = {}  # byte address of a 4-byte word -> warp
-    for warp in range(8):
-        wg, t0 = warp // 4, (warp % 4) * 32
+    for warp, rows in bands.items():
         chunks = [4 * g + jj for g in range(2) for jj in range(4)] if geglu else list(range(16))
-        for chunk in chunks:
-            for h in range(2):
-                addrs = [stage_offset(wg * 64 + acc_row(t0 + lane, 0) + 8 * h, chunk, swizzle) + 4 * (lane & 3) for lane in range(32)]
-                assert len({(a // 4) % 32 for a in addrs}) == 32, f"fragment store of chunk {chunk}: bank conflict"
-                for a in addrs:
-                    assert 0 <= a < 128 * 256 and a not in writer, "staging word written twice"
-                    writer[a] = warp
+        for r0 in rows:
+            for chunk in chunks:
+                for h in range(2):
+                    addrs = [stage_offset(r0 + acc_row(lane, 2 * h), chunk, swizzle) + 4 * (lane & 3) for lane in range(32)]
+                    assert len({(a // 4) % 32 for a in addrs}) == 32, f"fragment store of chunk {chunk}: bank conflict"
+                    for a in addrs:
+                        assert 0 <= a < 128 * 256 and a not in writer, "staging word written twice"
+                        writer[a] = warp
     want = {stage_offset(r, c, swizzle) + 4 * q for r in range(128) for c in range(cpr) for q in range(4)}
     assert set(writer) == want, "the fragment stores do not cover the tile"
     read = set()
-    for warp in range(8):
-        for i in range(8):
-            lanes = [(lane, 16 * warp + ((32 * i + lane) >> lg), (32 * i + lane) & (cpr - 1)) for lane in range(32)
-                     if ((32 * i + lane) >> lg) < 16]
-            for q in range(0, len(lanes), 8):
-                groups = {(stage_offset(r, c, swizzle) // 16) % 8 for _, r, c in lanes[q:q + 8]}
-                assert len(groups) == 8, "copy-out read: bank conflict inside a quarter warp"
-            for (l0, ra, ca), (l1, rb, cb) in zip(lanes, lanes[1:]):
-                assert (rb, cb) == ((ra, ca + 1) if ca + 1 < cpr else (ra + 1, 0)), "copy-out lanes are not consecutive chunks"
-            for _, r, c in lanes:
-                a = stage_offset(r, c, swizzle)
-                assert a not in read and all(writer[a + 4 * q] == warp for q in range(4)), "chunk read twice or by another warp"
-                read.add(a)
+    for warp, rows in bands.items():
+        for r0 in rows:
+            for i in range(8):
+                lanes = [(lane, r0 + ((32 * i + lane) >> lg), (32 * i + lane) & (cpr - 1)) for lane in range(32)
+                         if ((32 * i + lane) >> lg) < 16]
+                for q in range(0, len(lanes), 8):
+                    groups = {(stage_offset(r, c, swizzle) // 16) % 8 for _, r, c in lanes[q:q + 8]}
+                    assert len(groups) == 8, "copy-out read: bank conflict inside a quarter warp"
+                for (l0, ra, ca), (l1, rb, cb) in zip(lanes, lanes[1:]):
+                    assert (rb, cb) == ((ra, ca + 1) if ca + 1 < cpr else (ra + 1, 0)), "copy-out lanes are not consecutive chunks"
+                for _, r, c in lanes:
+                    a = stage_offset(r, c, swizzle)
+                    assert a not in read and all(writer[a + 4 * q] == warp for q in range(4)), "chunk read twice or by another warp"
+                    read.add(a)
     assert len(read) == 128 * cpr
     if not geglu:
         fetched = {}
-        for warp in range(8):
-            for i in range(8):
-                for lane in range(32):
-                    a = stage_offset(16 * warp + 2 * i + (lane >> 4), lane & 15, swizzle)
-                    assert a not in fetched and writer[a] == warp, "residual chunk fetched twice or by another warp"
-                    fetched[a] = warp
+        for warp, rows in bands.items():
+            for r0 in rows:
+                for i in range(8):
+                    for lane in range(32):
+                        a = stage_offset(r0 + 2 * i + (lane >> 4), lane & 15, swizzle)
+                        assert a not in fetched and writer[a] == warp, "residual chunk fetched twice or by another warp"
+                        fetched[a] = warp
         assert len(fetched) == 128 * 16
     return True
 
 
 def check_epilogue(geglu_pack, N_geglu=(128, 256, 2560)):
-    """gemm_wgmma_kernel's epilogue index arithmetic: (1) the accumulator layout maps the 128 threads x 64 registers of a
-    warpgroup one-to-one onto its 64 x 128 block; (2) GEGLU: the (h, gate) columns the kernel pairs (jh, jg = jh + 4 inside
-    each 64-column group; staged at chunk 4 g + jj, element cq of the tile row, i.e. output column n0 / 2 + 32 g + 8 jj + cq)
-    are the pairs geglu_pack interleaved, every output column written once; (3) out_row_offset of an up2 phase maps the
-    low-resolution pixels one-to-one onto the phase's pixels of the output; (4) the staging tile (check_epilogue_staging)."""
+    """The GEMM epilogues' index arithmetic: (1) the accumulator layout maps the 128 threads x 64 registers of a warpgroup
+    one-to-one onto its 64 x 128 block; (2) GEGLU (gemm_linear_ws_kernel): the (h, gate) columns the kernel pairs (jh,
+    jg = jh + 4 inside each 64-column group; staged at chunk 4 g + jj, element cq of the tile row, i.e. output column
+    n0 / 2 + 32 g + 8 jj + cq) are the pairs geglu_pack interleaved, every output column written once; (3) out_row_offset
+    of an up2 phase (gemm_wgmma_kernel) maps the low-resolution pixels one-to-one onto the phase's pixels of the output;
+    (4) the staging tile of each kernel's band ownership (check_epilogue_staging)."""
     import torch
     seen = {(acc_row(t, i), acc_col(t, i)) for t in range(128) for i in range(64)}
     assert len(seen) == 64 * 128 and all(0 <= r < 64 and 0 <= c < 128 for r, c in seen)
@@ -323,8 +344,8 @@ def check_epilogue(geglu_pack, N_geglu=(128, 256, 2560)):
                 rows.add((n * 2 * H + 2 * i + py) * (2 * W) + 2 * j + px)
             want = {(n * 2 * H + y) * (2 * W) + x for n in range(NF) for y in range(py, 2 * H, 2) for x in range(px, 2 * W, 2)}
             assert rows == want
-    for geglu in (False, True):
-        check_epilogue_staging(geglu)
+    for kernel, geglu in (("conv", False), ("linear", False), ("linear", True)):
+        check_epilogue_staging(kernel, geglu)
     return True
 
 
@@ -413,7 +434,7 @@ def simulate_rows_ring(rng: random.Random, n: int, stages: int, arrivals: int = 
 # ---------------------------------------------------------------------------------------------------------- persistent LINEAR GEMM
 def linear_ws_constants():
     """(stages, empty-barrier arrivals) of gemm_linear_ws_kernel's ring, as written in gemm_linear_ws.cu; also checks that the
-    tile schedule, the barrier parities, the turn taking and the staging layout are the ones the models below restate"""
+    tile schedule, the barrier parities and the turn taking are the ones the models below restate"""
     s = _src("gemm_linear_ws.cu")
     stages = int(re.search(r"constexpr int kStages = (\d+);", s).group(1))
     arrivals = int(re.search(r"mbar_init\(&empty\[s\], (\d+)\);", s).group(1))
@@ -422,8 +443,7 @@ def linear_ws_constants():
                  "const int g0 = i * nk;", "const int s = g % kStages, k0 = kb * BK;",
                  "mbar_wait<false>(&empty[s], ((g / kStages) - 1) & 1)", "mbar_wait<false>(&full[s], (g / kStages) & 1)",
                  "if (kb > 0) release(g - 1);", "release(g0 + nk - 1);", "if (wg == 1) named_bar_arrive(1, 256);",
-                 "if (t + gridDim.x < P.tiles) hand_over();", "tiles < sm_count_cached() ? tiles : sm_count_cached()",
-                 "return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));"):
+                 "if (t + gridDim.x < P.tiles) hand_over();", "tiles < sm_count_cached() ? tiles : sm_count_cached()"):
         assert rule in s, f"gemm_linear_ws.cu no longer contains {rule!r}: update the model"
     return stages, arrivals
 
