@@ -1,7 +1,9 @@
 // Shared by the two GEMM kernels: the launch parameters av2v_gemm_f16 validates and fills, the GEGLU activation and the
 // staged epilogue.
-//   gemm_wgmma.cu      : the conv modes (3 x 3, stride 2, up2 phase, temporal (3, 1, 1)), two CTAs per SM
-//   gemm_linear_ws.cu  : the LINEAR mode, persistent and warp-specialized
+//   gemm_linear_ws.cu  : persistent and warp-specialized, TMA-fed: the LINEAR mode, and the conv modes (3 x 3 stride 1, up2
+//                        phase, temporal (3, 1, 1)) whose 128-row tiles are each one box of the input (conv_ws_box)
+//   gemm_wgmma.cu      : the other conv geometries (stride 2, widths that do not divide 128, ...), cp.async-gathered, two
+//                        CTAs per SM
 #pragma once
 #include "host_util.cuh"
 #include "ptx.cuh"
@@ -63,9 +65,9 @@ __device__ __forceinline__ uint32_t stage_offset(int row, int chunk) {
   return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));
 }
 
-// The row mapping and the output tile differ by kernel, fixed at compile time so that neither kernel carries the other's:
-// kConv (gemm_wgmma.cu): the rows of an up2 phase are its pixels of the 2x output; otherwise (LINEAR, gemm_linear_ws.cu)
-// row m is out row m and a GEGLU tile is 128 x 64.
+// The row mapping and the output tile differ by A mode, fixed at compile time so that neither instantiation carries the
+// other's: kConv (gemm_wgmma.cu, gemm_ws_kernel<true>): the rows of an up2 phase are its pixels of the 2x output; otherwise
+// (LINEAR, gemm_ws_kernel<false>) row m is out row m and a GEGLU tile is 128 x 64.
 
 // element offset of output row m inside a slot of out / residual
 template <bool kConv>
@@ -156,7 +158,10 @@ __device__ __forceinline__ void copy_out_band(const GemmP& p, int slot, int m0, 
   }
 }
 
-// LINEAR-mode launch (gemm_linear_ws.cu) of `tiles` output tiles; p is validated and filled by av2v_gemm_f16
+// Launches of gemm_linear_ws.cu's persistent kernel on `tiles` output tiles; p is validated and filled by av2v_gemm_f16.
+// LINEAR mode; a conv mode whose tiles are each one box of its input (conv_ws_box returns true and the box).
 int gemm_linear_ws(const GemmP& p, int tiles, cudaStream_t stream);
+bool conv_ws_box(const GemmP& p, unsigned (&box)[3]);
+int gemm_conv_ws(const GemmP& p, const unsigned (&box)[3], int tiles, cudaStream_t stream);
 
 }  // namespace av2v

@@ -1,6 +1,7 @@
-// Persistent, warp-specialized GEMM of the LINEAR A mode (sm_90a): every nn.Linear / 1 x 1 conv of the UNet.
+// Persistent, warp-specialized GEMM (sm_90a): every nn.Linear / 1 x 1 conv of the UNet (LINEAR), and the 3 x 3 / up2-phase /
+// temporal convolutions whose 128-row tiles are each one TMA box of the input (conv_ws_box; the rest run on gemm_wgmma.cu).
 //
-//   out[m, n] = sum_k A[m, k] * W[n, k] + bias[n] + rowbias[m / rows_per_rowbias, n] + residual[m, n]   (or GEGLU)
+//   out[slot][m, n] = sum_k A[m, k] * W[n, k] + bias[n] + rowbias[m / rows_per_rowbias, n] + residual[slot][m, n]   (or GEGLU)
 //
 // These GEMMs have short K loops (K = C: 5 blocks of 64 at C = 320), so a CTA that runs one tile through load, K loop and
 // epilogue leaves the tensor cores idle for a large share of its life.  Here one CTA per SM walks a static tile schedule
@@ -20,12 +21,26 @@
 // producer refills the stage after the empty phase ((g / kStages) - 1) & 1 has completed (tools/kernel_models.py models
 // this schedule).
 //
+// The A source is a template parameter; only the producer's box coordinates and the epilogue's row mapping and slots differ.
+//   LINEAR: A is [M][lda] (two sources split at k_split), box (k0, m0).
+//   conv (kConv): K block kb lies inside one tap (Cin % 64 == 0), so it is a 64-channel slab of the channels-last input
+//     shifted by the tap: the input is a 4-D tensor (CONV3X3 [NF][H][W][chan], TCONV3 [B][F][HW][C]) whose box
+//     {64, bx, by, bn} holds exactly the 128 output rows of a tile, in row order (conv_ws_box picks it and refuses the
+//     geometries where no box does; a 3 x 3 conv's last tile may be ragged, its box running past the last frame).  Tile row m0 starts the box at (m0 % ax + x_off, m0 / ax % ay + y_off, m0 / (ax ay)),
+//     moved by the tap (kx, ky) = (tap % taps_w, tap / taps_w) of K block kb (tap = kb * 64 / Cin): the -1 offsets of a 3 x 3 conv, the phase offsets px - 1,
+//     py - 1 of an up2 phase, the frame offset kt - 1 of the temporal conv.  TMA zero-fill outside the tensor is the
+//     padding (out-of-image taps, the frames past either end of a clip, the channels past a_channels).  The smem image of a
+//     box with 128-byte rows is the same sw128 tile whatever its shape, and every block holds the values gemm_wgmma.cu's
+//     cp.async gather puts there, so K order, sum order and results are those of gemm_wgmma_kernel.
+//
 // Epilogue: gemm_common.cuh's staged epilogue, shared with gemm_wgmma_kernel; GEGLU pairs the h and gate columns that
 // geglu_pack interleaves, output tile 128 x 64.  Each consumer warpgroup has its own 32 KB staging tile; each warp owns two
 // bands (rows 16 w .. 16 w + 15 and 64 + 16 w .., one per accumulator) and fetches their residual chunks by cp.async
 // before its K loop, so a warp needs only __syncwarp: all of a warp's residual reads complete before its first store (a
 // residual that aliases out stays safe), and its copy-out reads complete before the next tile's residual fetch or stores
-// refill the tile.
+// refill the tile.  Conv with a residual in several slots (PnP conv injection) runs the slots one after another through
+// the one staging tile: fetch residual s (slot 0's before the K loop), epilogue, copy out to slot s, __syncwarp; without a
+// residual the one tile is copied to every slot.  An up2 phase writes its rows to the phase's pixels of the 2x output.
 #include "gemm_common.cuh"
 
 namespace av2v {
@@ -39,10 +54,11 @@ constexpr int kStageBytes = 2 * kTileBytes;
 constexpr int kStagingBytes = BM * BN * 2;             // 32 KB per consumer warpgroup
 constexpr int kSmemBytes = kStages * kStageBytes + 2 * kStagingBytes + 1024;
 
-struct LinWsP {
-  CUtensorMap ta, ta2, tw;  // A (columns [0, k_split)), second source (columns [k_split, K)), W [N][K]
+struct WsP {
+  CUtensorMap ta, ta2, tw;  // A (LINEAR: columns [0, k_split); conv: the input tensor), second source (columns [k_split, K)), W [N][K]
   GemmP g;
   int tiles;
+  int ax, ay, x_off, y_off, taps_w;  // conv: the box origin of tile row m0 and the taps per kernel row (see the top)
 };
 
 // GEGLU: h * gelu(gate) of the accumulator column pairs jh = 8 g + jj and jg = jh + 4 (the pairs geglu_pack interleaves)
@@ -77,7 +93,8 @@ __device__ __forceinline__ void geglu_epilogue(const GemmP& p, float (&d)[2][64]
   }
 }
 
-__global__ void __launch_bounds__(kThreads, 1) gemm_linear_ws_kernel(const __grid_constant__ LinWsP P) {
+template <bool kConv>
+__global__ void __launch_bounds__(kThreads, 1) gemm_ws_kernel(const __grid_constant__ WsP P) {
   const GemmP& p = P.g;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full[kStages], empty[kStages];
@@ -103,11 +120,23 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_linear_ws_kernel(const __gri
       int g = 0;
       for (int t = blockIdx.x; t < P.tiles; t += gridDim.x) {
         const int m0 = t / p.n_tiles * BM, n0 = t % p.n_tiles * BN;
+        int bx = 0, by = 0, bn = 0, c0 = 0, kx = 0;  // conv: the tile's box origin, block kb's channel and tap column
+        if constexpr (kConv) {
+          bx = m0 % P.ax + P.x_off;
+          by = m0 / P.ax % P.ay + P.y_off;
+          bn = m0 / (P.ax * P.ay);
+        }
         for (int kb = 0; kb < nk; ++kb, ++g) {
           const int s = g % kStages, k0 = kb * BK;
           if (g >= kStages) mbar_wait<false>(&empty[s], ((g / kStages) - 1) & 1);  // the consumer released block g - kStages
           mbar_arrive_expect_tx(&full[s], kStageBytes);
-          if (k0 < p.k_split) tma_load_4d(sA(s), &P.ta, &full[s], k0, m0, 0, 0);
+          if constexpr (kConv) {  // block kb = tap (ky, kx), channels c0 .. c0 + 63; walked without divisions
+            tma_load_4d(sA(s), &P.ta, &full[s], c0, bx + kx, by, bn);
+            if ((c0 += BK) == p.Cin) {
+              c0 = 0;
+              if (++kx == P.taps_w) kx = 0, ++by;
+            }
+          } else if (k0 < p.k_split) tma_load_4d(sA(s), &P.ta, &full[s], k0, m0, 0, 0);
           else tma_load_4d(sA(s), &P.ta2, &full[s], k0 - p.k_split, m0, 0, 0);
           tma_load_4d(sB(s), &P.tw, &full[s], k0, n0, 0, 0);
         }
@@ -136,7 +165,10 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_linear_ws_kernel(const __gri
     const int m0 = t / p.n_tiles * BM, n0 = t % p.n_tiles * BN;
     if (p.residual)
 #pragma unroll
-      for (int b = 0; b < 2; ++b) fetch_residual_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);
+      for (int b = 0; b < 2; ++b) {
+        if constexpr (kConv) fetch_residual_band<true>(p, 0, m0, n0, r0 + 64 * b, staging);
+        else fetch_residual_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);
+      }
     cp_async_commit();
 #pragma unroll
     for (int h = 0; h < 2; ++h)
@@ -166,21 +198,57 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_linear_ws_kernel(const __gri
     reg_fence(d[1]);
     release(g0 + nk - 1);
 
-    cp_async_wait<0>();
-    __syncwarp();  // the residual chunks this warp's lanes fetched for each other have landed
-    if (p.geglu) geglu_epilogue(p, d, n0, staging);
-    else epilogue_bands<2>(p, d, m0, n0, r0, staging);
-    __syncwarp();
+    if constexpr (kConv) {
+      // d stays live across the slots: the slot and copy-out loops stay rolled so that the copy-out's addresses fit beside it
+      const int n_res = p.residual ? p.n_slots : 1;  // distinct tiles: without a residual every slot stores the same one
+#pragma unroll 1
+      for (int sl = 0; sl < n_res; ++sl) {
+        if (sl > 0) {  // the copy-out of slot sl - 1 has read the warp's rows (__syncwarp below)
 #pragma unroll
-    for (int b = 0; b < 2; ++b) copy_out_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);
-    __syncwarp();  // every lane's copy-out reads are done before the next tile refills the warp's rows
+          for (int b = 0; b < 2; ++b) fetch_residual_band<true>(p, sl, m0, n0, r0 + 64 * b, staging);
+          cp_async_commit();
+        }
+        cp_async_wait<0>();
+        __syncwarp();  // the residual chunks this warp's lanes fetched for each other have landed
+        epilogue_bands<2>(p, d, m0, n0, r0, staging);
+        __syncwarp();
+#pragma unroll 1
+        for (int o = p.residual ? sl : 0; o < (p.residual ? sl + 1 : p.n_slots); ++o)
+#pragma unroll 1
+          for (int b = 0; b < 2; ++b) copy_out_band<true>(p, o, m0, n0, r0 + 64 * b, staging);
+        __syncwarp();  // every lane's copy-out reads are done before the next slot or tile refills the warp's rows
+      }
+    } else {
+      cp_async_wait<0>();
+      __syncwarp();  // the residual chunks this warp's lanes fetched for each other have landed
+      if (p.geglu) geglu_epilogue(p, d, n0, staging);
+      else epilogue_bands<2>(p, d, m0, n0, r0, staging);
+      __syncwarp();
+#pragma unroll
+      for (int b = 0; b < 2; ++b) copy_out_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);
+      __syncwarp();  // every lane's copy-out reads are done before the next tile refills the warp's rows
+    }
   }
+}
+
+template <bool kConv>
+int launch_ws(const WsP& P, cudaStream_t stream) {
+  static bool attr_set = false;  // one per instantiation
+  if (!attr_set) {
+    AV2V_CHECK_CUDA(cudaFuncSetAttribute(gemm_ws_kernel<kConv>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+    attr_set = true;
+  }
+  const int tiles = P.tiles;
+  const int grid = static_cast<int>(tiles < sm_count_cached() ? tiles : sm_count_cached());
+  gemm_ws_kernel<kConv><<<grid, kThreads, kSmemBytes, stream>>>(P);
+  AV2V_CHECK_CUDA(cudaGetLastError());
+  return AV2V_OK;
 }
 
 }  // namespace
 
 int gemm_linear_ws(const GemmP& g, int tiles, cudaStream_t stream) {
-  LinWsP P{};
+  WsP P{};
   P.g = g;
   if (int e = encode_rows_map(&P.ta, g.a, g.k_split, g.M, 1, 1, g.lda, 0, BM)) return e;
   P.ta2 = P.ta;
@@ -188,15 +256,67 @@ int gemm_linear_ws(const GemmP& g, int tiles, cudaStream_t stream) {
     if (int e = encode_rows_map(&P.ta2, g.a2, g.K - g.k_split, g.M, 1, 1, g.lda2, 0, BM)) return e;
   if (int e = encode_rows_map(&P.tw, g.w, g.K, g.N, 1, 1, g.K, 0, BN)) return e;
   P.tiles = tiles;
-  static bool attr_set = false;
-  if (!attr_set) {
-    AV2V_CHECK_CUDA(cudaFuncSetAttribute(gemm_linear_ws_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    attr_set = true;
+  return launch_ws<false>(P, stream);
+}
+
+// A conv runs here iff the 128 output rows of every tile are one box of its input, in row order:
+//   CONV3X3, stride 1 or an up2 phase (the GEMM rows are the NF x Ho x Wo pixels, Ho x Wo the input's extent): Wo divides
+//     128 and either 128 divides Ho Wo (box Wo x 128 / Wo x 1) or Ho Wo divides 128 (whole frames, box Wo x Ho x
+//     128 / (Ho Wo)).  The frame is the outermost dimension, so the box of a ragged last tile runs past frame NF - 1 into
+//     zeros, on rows past M that are never stored;
+//   TCONV3 (rows B x F x HW): 128 divides HW (box 128 x 1) or HW divides 128 and 128 / HW divides F (box HW x 128 / HW):
+//     a box past the last frame of a clip would hold zeros where the tile's rows are the next clip's first frame.
+// box = {bx, by, bn}, the box extents past the 64 channels.
+bool conv_ws_box(const GemmP& p, unsigned (&box)[3]) {
+  if (p.mode == AV2V_A_CONV3X3) {
+    const int hw = p.Ho * p.Wo;
+    if (p.stride != 1 || BM % p.Wo != 0) return false;
+    if (hw >= BM) {
+      if (hw % BM != 0) return false;
+      box[0] = p.Wo, box[1] = BM / p.Wo, box[2] = 1;
+    } else {
+      if (BM % hw != 0) return false;
+      box[0] = p.Wo, box[1] = p.Ho, box[2] = BM / hw;
+    }
+    return true;
   }
-  const int grid = static_cast<int>(tiles < sm_count_cached() ? tiles : sm_count_cached());
-  gemm_linear_ws_kernel<<<grid, kThreads, kSmemBytes, stream>>>(P);
-  AV2V_CHECK_CUDA(cudaGetLastError());
-  return AV2V_OK;
+  if (p.mode == AV2V_A_TCONV3) {
+    if (p.HW % BM == 0) box[0] = BM, box[1] = 1, box[2] = 1;
+    else if (BM % p.HW == 0 && p.F % (BM / p.HW) == 0) box[0] = p.HW, box[1] = BM / p.HW, box[2] = 1;
+    else return false;
+    return true;
+  }
+  return false;
+}
+
+int gemm_conv_ws(const GemmP& g, const unsigned (&box)[3], int tiles, cudaStream_t stream) {
+  WsP P{};
+  P.g = g;
+  using u64 = unsigned long long;
+  const unsigned b4[4] = {64, box[0], box[1], box[2]};
+  if (g.mode == AV2V_A_CONV3X3) {  // [NF][Hin][Win][chan]; stride 1, so Hin = Ho, Win = Wo
+    const u64 row = static_cast<u64>(g.chan) * 2, plane = row * g.Win * g.Hin;
+    const u64 dims[4] = {static_cast<u64>(g.chan), static_cast<u64>(g.Win), static_cast<u64>(g.Hin),
+                         static_cast<u64>(g.M / (g.Ho * g.Wo))};
+    const u64 strides[3] = {row, row * g.Win, plane};
+    if (int e = encode_map_4d(&P.ta, g.a, dims, strides, b4)) return e;
+    P.ax = g.Wo, P.ay = g.Ho, P.taps_w = g.taps_w;
+    P.x_off = g.up2 ? g.px - 1 : -1;
+    P.y_off = g.up2 ? g.py - 1 : -1;
+  } else {  // TCONV3: [B][F][HW][Cin]
+    const u64 row = static_cast<u64>(g.Cin) * 2;
+    const u64 dims[4] = {static_cast<u64>(g.Cin), static_cast<u64>(g.HW), static_cast<u64>(g.F),
+                         static_cast<u64>(g.M / (g.F * g.HW))};
+    const u64 strides[3] = {row, row * g.HW, row * g.HW * g.F};
+    if (int e = encode_map_4d(&P.ta, g.a, dims, strides, b4)) return e;
+    P.ax = g.HW, P.ay = g.F, P.taps_w = 1;
+    P.x_off = 0;
+    P.y_off = -1;
+  }
+  P.ta2 = P.ta;
+  if (int e = encode_rows_map(&P.tw, g.w, g.K, g.N, 1, 1, g.K, 0, BN)) return e;
+  P.tiles = tiles;
+  return launch_ws<true>(P, stream);
 }
 
 }  // namespace av2v

@@ -1,5 +1,8 @@
-// wgmma GEMM core of the I2VGen-XL UNet hot path (sm_90a): the convolutions.  av2v_gemm_f16 validates every call and sends
-// the LINEAR mode to gemm_linear_ws.cu's persistent kernel; the conv modes run here.
+// wgmma GEMM core of the I2VGen-XL UNet hot path (sm_90a): the convolutions gemm_linear_ws.cu's persistent kernel does not
+// take.  av2v_gemm_f16 validates every call the same way whichever kernel runs it, then sends the LINEAR mode, and every
+// conv whose 128-row tiles are each one TMA box of its input (conv_ws_box: 3 x 3 stride 1 and up2 phases at widths that
+// divide 128, temporal convs whose tiles hold whole frames of one clip), to gemm_linear_ws.cu; the rest (stride 2, widths
+// such as 27 or 88, temporal convs whose frame count the box does not divide) run here.
 //
 //   out[slot][m, n] = sum_k A[m, k] * W[n, k] + bias[n] + rowbias[m / rows_per_rowbias, n] + residual[slot][m, n]
 //
@@ -268,6 +271,8 @@ extern "C" int av2v_gemm_f16(const av2v_gemm_args* a, av2v_stream_t stream_) {
   const long long tiles = static_cast<long long>((a->M + BM - 1) / BM) * p.n_tiles;
   AV2V_REQUIRE(tiles < (1ll << 31), AV2V_ENOSUP, "gemm: too many tiles");
   if (p.mode == AV2V_A_LINEAR) return gemm_linear_ws(p, static_cast<int>(tiles), stream);
+  unsigned box[3];
+  if (conv_ws_box(p, box)) return gemm_conv_ws(p, box, static_cast<int>(tiles), stream);
   static bool attr_set = false;
   if (!attr_set) {
     AV2V_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));

@@ -39,7 +39,10 @@ inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 int sm_count_cached();  // abi.cu
 
-// 4-D fp16 tensor map for TMA tile loads: boxes of 64 columns x box_rows rows, 128-byte swizzle (abi.cu)
+// 4-D fp16 tensor maps for TMA tile loads, 128-byte swizzle, zeros outside the tensor (abi.cu): any dims, byte strides and
+// box with 64-element rows; and the rows map of the GEMM and attention operands, boxes of 64 columns x box_rows rows
+int encode_map_4d(CUtensorMap* map, const void* base, const unsigned long long (&dims)[4],
+                  const unsigned long long (&strides)[3], const unsigned (&box)[4]);
 int encode_rows_map(CUtensorMap* map, const void* base, int cols, int tokens, int seqs, int branches, int ld,
                     long long branch_stride, int box_rows);
 

@@ -81,11 +81,26 @@ def _cases(dev):
                 cases[f"conv3x3+res 3 slots {Ms}x{C}x{9 * C}"] = (
                     lambda xi=xi[:F], w=wc, b=bias, r=res, o=out, s=Ms * C: ops.conv3x3(xi, w, bias=b, residual=r.view(3, -1, r.shape[1]), out=o.view(3, -1, o.shape[1]), n_slots=3, slot_stride=s),
                     2 * Ms * C * 9 * C, 2 * (Ms * C + 9 * C * C + 2 * 3 * Ms * C))
+            # resnet conv1: 3 x 3 conv + bias + the per-frame time embedding (rowbias), no residual
+            cases[f"conv3x3+rowbias {M}x{C}x{9 * C}"] = (lambda xi=xi, w=wc, b=bias, t=tproj, o=out, r=hw * hw: ops.conv3x3(xi, w, bias=b, rowbias=t, rows_per_rowbias=r, out=o),
+                                                        2 * M * C * 9 * C, 2 * (M * C + 9 * C * C + B * F * C + M * C))
             if lvl == 0:
                 x2 =torch.randn(B * F, hw, hw, 2 * C, device=dev).half()
                 wc2 = _w(C, 18 * C, dev)
                 cases[f"conv3x3 {M}x{C}x{18 * C}"] = (lambda xi=x2, w=wc2, b=bias, o=out: ops.conv3x3(xi, w, bias=b, out=o),
                                                      2 * M * C * 18 * C, 2 * (M * 2 * C + 18 * C * C + M * C))
+        # the 8 x 8 level (mid block and down block 3): two frames per 128-row tile
+        hw, C = 8, 1280
+        M = B * F * hw * hw
+        x8 = torch.randn(B * F, hw, hw, C, device=dev).half()
+        r8 = torch.randn(M, C, device=dev).half()
+        o8 = torch.empty(M, C, device=dev).half()
+        b8 = (torch.randn(C, device=dev) * 0.1).half()
+        wc8, wt8 = _w(C, 9 * C, dev), _w(C, 3 * C, dev)
+        cases[f"conv3x3+res {M}x{C}x{9 * C}"] = (lambda xi=x8, w=wc8, b=b8, r=r8, o=o8: ops.conv3x3(xi, w, bias=b, residual=r, out=o),
+                                                2 * M * C * 9 * C, 2 * (M * C + 9 * C * C + 2 * M * C))
+        cases[f"tconv3 {M}x{C}x{3 * C}"] = (lambda x3=x8.view(B, F * hw * hw, C), w=wt8, b=b8, o=o8, hw=hw: ops.tconv3(x3, w, F, hw * hw, bias=b, out=o.view(x3.shape)),
+                                           2 * M * C * 3 * C, 2 * (M * C + 3 * C * C + M * C))
         # up-sampling (nearest x 2 + 3 x 3 conv as four phase GEMMs, K = 4 Cin) into levels 1 and 0's resolutions
         for hw, C in ((8, 1280), (16, 1280), (32, 640)):
             Ml = B * F * hw * hw
@@ -150,6 +165,9 @@ def main():
     linear = [c for c in cases if c.split()[0] in ("linear", "linear+res", "linear+rowbias", "geglu")]
     print("sum over the linear-mode shapes:", ", ".join(f"{n if n == 'this' else os.path.basename(os.path.dirname(os.path.abspath(n)))} "
                                                         f"{sum(statistics.median(times[(n, c)]) for c in linear):.1f} us" for n in libs))
+    conv = [c for c in cases if c not in linear]
+    print("sum over the conv-mode shapes:", ", ".join(f"{n if n == 'this' else os.path.basename(os.path.dirname(os.path.abspath(n)))} "
+                                                      f"{sum(statistics.median(times[(n, c)]) for c in conv):.1f} us" for n in libs))
     differ = [c for c in cases if not equal[c]]
     print("outputs torch.equal across builds:", "every shape" if not differ else f"NO, differ on {differ}")
     print(json.dumps(rows))

@@ -232,7 +232,7 @@ def stage_offset(row, chunk, swizzle=True):
 def epilogue_bands(kernel: str):
     """warp -> first tile rows of the bands it owns in one staging tile: the rows its accumulators hold (acc_row).
     conv (gemm_wgmma_kernel): 8 warps, warpgroup wg's one accumulator holds tile rows 64 wg .. 64 wg + 63.
-    linear (gemm_linear_ws_kernel): a consumer warpgroup's own tile, 4 warps, accumulator b holds tile rows 64 b .. 64 b + 63."""
+    linear (gemm_ws_kernel, LINEAR and conv alike): a consumer warpgroup's own tile, 4 warps, accumulator b holds tile rows 64 b .. 64 b + 63."""
     if kernel == "conv":
         return {w: [64 * (w // 4) + acc_row(32 * (w % 4), 0)] for w in range(8)}
     assert kernel == "linear", kernel
@@ -249,7 +249,7 @@ def check_epilogue_staging(kernel: str, geglu: bool = False, swizzle: bool = Tru
     (whole 128-byte lines of the output row), and every chunk is read exactly once BY THE WARP THAT WROTE IT — the kernels
     order the two with __syncwarp only.  (3) The residual cp.async pattern (2 rows x 16 chunks per instruction) fetches
     every chunk once, again in the warp that consumes it.  swizzle=False is the negative control."""
-    assert not (geglu and kernel == "conv"), "GEGLU runs on gemm_linear_ws_kernel only"
+    assert not (geglu and kernel == "conv"), "GEGLU runs on gemm_ws_kernel<false> only"
     src = _src("gemm_common.cuh")
     assert "return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));" in src, "stage_offset changed: update the model"
     for f, rule in (("gemm_wgmma.cu", "const int r0 = 16 * (threadIdx.x >> 5);"),
@@ -304,7 +304,7 @@ def check_epilogue_staging(kernel: str, geglu: bool = False, swizzle: bool = Tru
 
 def check_epilogue(geglu_pack, N_geglu=(128, 256, 2560)):
     """The GEMM epilogues' index arithmetic: (1) the accumulator layout maps the 128 threads x 64 registers of a warpgroup
-    one-to-one onto its 64 x 128 block; (2) GEGLU (gemm_linear_ws_kernel): the (h, gate) columns the kernel pairs (jh,
+    one-to-one onto its 64 x 128 block; (2) GEGLU (gemm_ws_kernel<false>): the (h, gate) columns the kernel pairs (jh,
     jg = jh + 4 inside each 64-column group; staged at chunk 4 g + jj, element cq of the tile row, i.e. output column
     n0 / 2 + 32 g + 8 jj + cq) are the pairs geglu_pack interleaved, every output column written once; (3) out_row_offset
     of an up2 phase (gemm_wgmma_kernel) maps the low-resolution pixels one-to-one onto the phase's pixels of the output;
@@ -433,7 +433,7 @@ def simulate_rows_ring(rng: random.Random, n: int, stages: int, arrivals: int = 
 
 # ---------------------------------------------------------------------------------------------------------- persistent LINEAR GEMM
 def linear_ws_constants():
-    """(stages, empty-barrier arrivals) of gemm_linear_ws_kernel's ring, as written in gemm_linear_ws.cu; also checks that the
+    """(stages, empty-barrier arrivals) of gemm_ws_kernel's ring, as written in gemm_linear_ws.cu; also checks that the
     tile schedule, the barrier parities and the turn taking are the ones the models below restate"""
     s = _src("gemm_linear_ws.cu")
     stages = int(re.search(r"constexpr int kStages = (\d+);", s).group(1))
@@ -470,7 +470,7 @@ def linear_ws_schedule(tiles: int, sms: int, off_by_one: bool = False):
 
 def simulate_linear_ws(rng: random.Random, n_tiles: int, nk: int, stages: int, arrivals: int = 4, release: bool = True,
                        wrong_parity: str = "", pingpong: bool = True, early_refill: bool = False):
-    """one CTA of gemm_linear_ws_kernel with n_tiles tiles of nk K blocks.  Producer: block g = i * nk + kb in stage g % S,
+    """one CTA of gemm_ws_kernel with n_tiles tiles of nk K blocks.  Producer: block g = i * nk + kb in stage g % S,
     waits empty with parity ((g / S) - 1) & 1 (g >= S), then TMA (full completes when the bytes land).  Consumer w takes local
     tiles i = w, w + 2, ...: fetches the tile's residual into its staging tile (cp.async), waits for its turn (warpgroup 1
     arrives on warpgroup 0's barrier first; a warpgroup hands over after issuing its last MMA when a tile follows), per block
@@ -549,4 +549,153 @@ def simulate_linear_ws(rng: random.Random, n_tiles: int, nk: int, stages: int, a
     assert [w for _, _, w in loops] == [i % 2 for i in range(n_tiles)], "the K loops do not take turns 0, 1, 0, 1, ..."
     for (s0, e0, _), (s1, _, _) in zip(loops, loops[1:]):
         assert e0 <= s1, "the K loops of the two consumers overlap"
+    return True
+
+
+# ---------------------------------------------------------------------------------------------------------- conv A tiles by TMA
+def conv_ws_rules():
+    """checks that gemm_linear_ws.cu / gemm_wgmma.cu still dispatch the conv modes, place each box and walk the taps as
+    conv_ws_box, conv_box_origin and tma_a_tile restate them"""
+    s = _src("gemm_linear_ws.cu")
+    for rule in ("if (p.stride != 1 || BM % p.Wo != 0) return false;", "if (hw % BM != 0) return false;",
+                 "box[0] = p.Wo, box[1] = BM / p.Wo, box[2] = 1;", "if (BM % hw != 0) return false;",
+                 "box[0] = p.Wo, box[1] = p.Ho, box[2] = BM / hw;", "if (p.HW % BM == 0) box[0] = BM, box[1] = 1, box[2] = 1;",
+                 "else if (BM % p.HW == 0 && p.F % (BM / p.HW) == 0) box[0] = p.HW, box[1] = BM / p.HW, box[2] = 1;",
+                 "P.ax = g.Wo, P.ay = g.Ho, P.taps_w = g.taps_w;", "P.x_off = g.up2 ? g.px - 1 : -1;",
+                 "P.y_off = g.up2 ? g.py - 1 : -1;", "P.ax = g.HW, P.ay = g.F, P.taps_w = 1;", "P.x_off = 0;", "P.y_off = -1;",
+                 "const unsigned b4[4] = {64, box[0], box[1], box[2]};",
+                 "bx = m0 % P.ax + P.x_off;", "by = m0 / P.ax % P.ay + P.y_off;", "bn = m0 / (P.ax * P.ay);",
+                 "tma_load_4d(sA(s), &P.ta, &full[s], c0, bx + kx, by, bn);", "if ((c0 += BK) == p.Cin) {",
+                 "if (++kx == P.taps_w) kx = 0, ++by;"):
+        assert rule in s, f"gemm_linear_ws.cu no longer contains {rule!r}: update the model"
+    assert "if (conv_ws_box(p, box)) return gemm_conv_ws(p, box, static_cast<int>(tiles), stream);" in _src("gemm_wgmma.cu")
+    return True
+
+
+def conv_geometry(mode: str, **g):
+    """the GemmP fields av2v_gemm_f16 fills for a conv call.  mode "conv": NF, H, W, Cin, chan (a_channels, default Cin),
+    stride (1), phase (0: plain; 1..4: up2 phase (py, px) = ((phase - 1) >> 1, (phase - 1) & 1)); mode "tconv": B, F, HW,
+    Cin"""
+    if mode == "conv":
+        ph, st = g.get("phase", 0), g.get("stride", 1)
+        d = dict(mode=mode, NF=g["NF"], Hin=g["H"], Win=g["W"], Ho=g["H"] // st, Wo=g["W"] // st, stride=st, Cin=g["Cin"],
+                 chan=g.get("chan", g["Cin"]), up2=int(ph > 0), py=(ph - 1) >> 1 if ph else 0, px=(ph - 1) & 1 if ph else 0,
+                 taps_w=2 if ph else 3)
+        d.update(M=d["NF"] * d["Ho"] * d["Wo"], K=(4 if ph else 9) * d["Cin"])
+    else:
+        d = dict(mode=mode, B=g["B"], F=g["F"], HW=g["HW"], Cin=g["Cin"], M=g["B"] * g["F"] * g["HW"], K=3 * g["Cin"])
+    return d
+
+
+def conv_ws_box(p):
+    """gemm_linear_ws.cu conv_ws_box: (bx, by, bn), or None when the conv stays on gemm_wgmma_kernel"""
+    if p["mode"] == "conv":
+        hw = p["Ho"] * p["Wo"]
+        if p["stride"] != 1 or 128 % p["Wo"]:
+            return None
+        if hw >= 128:
+            return None if hw % 128 else (p["Wo"], 128 // p["Wo"], 1)
+        return None if 128 % hw else (p["Wo"], p["Ho"], 128 // hw)
+    if p["HW"] % 128 == 0:
+        return (128, 1, 1)
+    if 128 % p["HW"] == 0 and p["F"] % (128 // p["HW"]) == 0:
+        return (p["HW"], 128 // p["HW"], 1)
+    return None
+
+
+def _conv_tensor(p):
+    """the 4-D tensor gemm_conv_ws describes (dims innermost first) and its box origin terms ax, ay, x_off, y_off, taps_w"""
+    if p["mode"] == "conv":
+        return ((p["chan"], p["Win"], p["Hin"], p["NF"]), p["Wo"], p["Ho"], p["px"] - 1 if p["up2"] else -1,
+                p["py"] - 1 if p["up2"] else -1, p["taps_w"])
+    return (p["Cin"], p["HW"], p["F"], p["B"]), p["HW"], p["F"], 0, -1, 1
+
+
+def tma_a_tile(p, x, m0, box, x_off=None, y_off=None, swap_phase=False):
+    """the A tiles of every K block of the tile at row m0 as the producer loads them: the box origin of the tile, the tap
+    walk (c0, kx, by) per block, and TMA's element placement (box element (i0, i1, i2, i3) -> tile row i1 + bx (i2 + by i3),
+    column i0; zero outside the tensor).  x: the flat input, dense in the tensor's dims.  Returns [num_kb, 128, 64].
+    x_off / y_off override the tap offsets; swap_phase exchanges the phase offsets (negative controls)."""
+    import numpy as np
+    dims, ax, ay, xo, yo, taps_w = _conv_tensor(p)
+    if swap_phase:
+        xo, yo = yo, xo
+    xo = xo if x_off is None else x_off
+    yo = yo if y_off is None else y_off
+    bx_, by_, bn_ = box
+    assert bx_ * by_ * bn_ == 128 and max(box) <= 256
+    i0, i1, i2, i3 = np.meshgrid(np.arange(64), np.arange(bx_), np.arange(by_), np.arange(bn_), indexing="ij")
+    row = (i1 + bx_ * (i2 + by_ * i3)).ravel()
+    col = i0.ravel()
+    bx, by, bn = m0 % ax + xo, m0 // ax % ay + yo, m0 // (ax * ay)
+    c0 = kx = 0
+    tiles = []
+    for _ in range(p["K"] // 64):
+        c = np.stack([(c0 + i0).ravel(), (bx + kx + i1).ravel(), (by + i2).ravel(), (bn + i3).ravel()])
+        ok = np.all((c >= 0) & (c < np.array(dims)[:, None]), axis=0)
+        flat = ((c[3] * dims[2] + c[2]) * dims[1] + c[1]) * dims[0] + c[0]
+        t = np.zeros((128, 64), x.dtype)
+        t[row, col] = np.where(ok, x[np.where(ok, flat, 0)], 0)
+        tiles.append(t)
+        c0 += 64
+        if c0 == p["Cin"]:
+            c0 = 0
+            kx += 1
+            if kx == taps_w:
+                kx, by = 0, by + 1
+    return np.stack(tiles)
+
+
+def gather_a_tile(p, x, m0):
+    """gemm_wgmma.cu a_rows_init + load_stage: the A tiles of every K block of the tile at row m0 as the cp.async gather
+    fills them (16-byte chunks, zero-filled out of the image / clip, past a_channels and past M).  [num_kb, 128, 64]"""
+    import numpy as np
+    r = np.arange(128)
+    m = m0 + r
+    live = m < p["M"]
+    ch = np.arange(64)
+    tiles = []
+    for kb in range(p["K"] // 64):
+        k0 = kb * 64
+        if p["mode"] == "conv":
+            ox, t = m % p["Wo"], m // p["Wo"]
+            oy, n = t % p["Ho"], t // p["Ho"]
+            y0 = oy - 1 + p["py"] if p["up2"] else oy * p["stride"] - 1
+            x0 = ox - 1 + p["px"] if p["up2"] else ox * p["stride"] - 1
+            tap = k0 // p["Cin"]
+            c = k0 - tap * p["Cin"] + ch
+            ky, kx = tap // p["taps_w"], tap % p["taps_w"]
+            y, xx = y0 + ky, x0 + kx
+            v = live[:, None] & (c[None, :] // 8 * 8 < p["chan"]) & ((y >= 0) & (y < p["Hin"]) & (xx >= 0) & (xx < p["Win"]))[:, None]
+            src = ((n * p["Hin"] + y) * p["Win"] + xx)[:, None] * p["chan"] + c[None, :]
+        else:
+            kt = k0 // p["Cin"]
+            c = k0 - kt * p["Cin"] + ch
+            fr = (m % (p["F"] * p["HW"])) // p["HW"]
+            f = fr + kt - 1
+            v = live[:, None] & ((f >= 0) & (f < p["F"]))[:, None] & np.ones(64, bool)[None, :]
+            src = (m + (kt - 1) * p["HW"])[:, None] * p["Cin"] + c[None, :]
+        tiles.append(np.where(v, x[np.where(v, src, 0)], 0))
+    return np.stack(tiles)
+
+
+def check_conv_tma_tiles(mode: str, box=None, **kw):
+    """every A tile of every K block of every output tile: the producer's TMA boxes hold exactly what gemm_wgmma_kernel's
+    gather loads.  box: force this box (default: conv_ws_box, which must accept the geometry); other keywords of
+    tma_a_tile (x_off, y_off, swap_phase) break one rule for the negative controls."""
+    import numpy as np
+    geo = {k: v for k, v in kw.items() if k not in ("x_off", "y_off", "swap_phase")}
+    bad = {k: v for k, v in kw.items() if k in ("x_off", "y_off", "swap_phase")}
+    p = conv_geometry(mode, **geo)
+    box = box or conv_ws_box(p)
+    assert box is not None, f"{mode} {geo}: conv_ws_box refuses the geometry"
+    dims = _conv_tensor(p)[0]
+    n = dims[0] * dims[1] * dims[2] * dims[3]
+    x = np.arange(1, n + 1, dtype=np.int64)  # every element distinct and nonzero: a zero is padding
+    for m0 in range(0, p["M"], 128):
+        want, got = gather_a_tile(p, x, m0), tma_a_tile(p, x, m0, box, **bad)
+        if not np.array_equal(want, got):
+            kb, r, c = (int(i[0]) for i in np.nonzero(want != got))
+            raise AssertionError(f"{mode} {geo}: tile row {m0} K block {kb} row {r} col {c}: TMA box holds {got[kb, r, c]}, "
+                                 f"the gather {want[kb, r, c]}")
     return True
