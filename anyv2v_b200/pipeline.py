@@ -2,7 +2,7 @@
 
 Drop-in for the hot loops of the reference's ``I2VGenXLPipeline`` (i2vgen-xl/pipelines/pipeline_i2vgen_xl.py):
   invert            :1197-1439 (loop :1385-1433)
-  sample_with_pnp   :892-1195  (loop :1131-1179)
+  sample_with_pnp   :892-1195  (loop :1131-1179; also eta > 0)
   __call__          :652-890   (loop :839-874; also eta > 0)
 with the same keyword surface for everything that reaches the loops.  Differences, none of which changes a result:
   * no host sync inside the loop: timesteps are Python ints (the reference calls ``t.item()`` at :1143 and runs
@@ -82,6 +82,7 @@ def _loop_state(latents, timesteps, scheduler, guidance_scale: float, device, et
     st.coef_table = scheduler.coefficient_table(timesteps, guidance_scale, device, eta=eta)
     st.g_t = torch.zeros(1, device=device, dtype=torch.int64)
     st.g_coef = torch.zeros(st.coef_table.shape[-1], device=device, dtype=torch.float32)
+    st.g_noise = torch.zeros_like(st.latents) if eta > 0 else None  # the step noise of eta > 0 (I2VGenXLPipeline._draw_noise)
     st.iterations = {}  # graph key of the loop -> _GraphedIteration
     st.graph_pool = torch.cuda.graph_pool_handle() if st.latents.is_cuda else None
     return st
@@ -383,7 +384,6 @@ class I2VGenXLPipeline:
         logger.info("Sampling starts from latents_at_t=%s", ts[0] if ts else None)
         st = _loop_state(latents, ts, self.scheduler, guidance_scale if cfg else 1.0, dev, eta=float(eta), cond=cond,
                          generator=generator, n_videos=n_videos)
-        st.g_noise = torch.zeros_like(st.latents) if st.eta > 0 else None
         # uncond and cond of one video have the same latents, image latents, fps and timestep: they share the UNet prefix
         # up to the first cross-attention.  With N > 1 the last two branches are different videos.
         st.shared_prefix = cfg and n_videos == 1
@@ -402,14 +402,19 @@ class I2VGenXLPipeline:
         st.body = body
         return st
 
-    def call_step(self, st, i: int):
-        """One iteration of the sampling loop (pipeline :839-874): UNet on [uncond, cond] -> CFG + DDIM step, in place.
-        With eta > 0 the step noise is drawn here, eagerly and in the reference's [N*F, C, h, w] order (:864-868), so that
-        the draws from ``generator`` are those of the reference, and copied into the buffer the (captured) step reads."""
+    @staticmethod
+    def _draw_noise(st):
+        """With eta > 0, the variance noise of one step: drawn eagerly from ``st.generator`` in the reference's
+        [N*F, C, h, w] order (the step runs on the frame-major reshape, pipeline :864-868 / :1168-1176), so that the draws
+        are those of the reference, and copied into the buffer ``st.g_noise`` the (captured) step reads.  Nothing with eta = 0."""
         if st.g_noise is not None:
             n, c, f, h, w = st.latents.shape
             z = randn_tensor((n * f, c, h, w), generator=st.generator, device=st.latents.device, dtype=st.latents.dtype)
             st.g_noise.copy_(z.view(n, f, c, h, w).permute(0, 2, 1, 3, 4))
+
+    def call_step(self, st, i: int):
+        """One iteration of the sampling loop (pipeline :839-874): UNet on [uncond, cond] -> CFG + DDIM step, in place."""
+        self._draw_noise(st)
         return self._run(st, i, (self.unet.freeu_state(), st.eta > 0), lambda: st.body)
 
     # -- phase 1 --------------------------------------------------------------------------------------------------
@@ -499,7 +504,9 @@ class I2VGenXLPipeline:
                         callback: Optional[Callable] = None, max_steps: Optional[int] = None,
                         decode_chunk_size: Optional[int] = None, **_ignored):
         """PnP edit loop (pipeline :1131-1179) over the branches [source, uncond, cond]; `output_type` "latent" returns
-        the latents, "pt" / "np" / "pil" decode them with the attached VAE (:1180-1194)."""
+        the latents, "pt" / "np" / "pil" decode them with the attached VAE (:1180-1194).  ``eta > 0`` edits stochastically:
+        every step, dead-source steps included, adds sigma_t * z with z drawn from ``generator`` as diffusers' DDIMScheduler
+        draws it (:1126, :1173)."""
         # raw inputs (the reference's only interface, :1014-1094) are encoded once per clip when encoders / VAE are attached;
         # the source first frame is cropped to the size of the edited one
         height, width = self._size_of(image, height, width)
@@ -513,18 +520,23 @@ class I2VGenXLPipeline:
         st = self.prepare_edit(latents, prompt_embeds, negative_prompt_embeds, ddim_inv_prompt_embeds, image_embeddings,
                                image_latents, ddim_inv_image_embeddings, ddim_inv_image_latents, target_fps,
                                num_inference_steps, guidance_scale, ddim_init_latents_t_idx, ddim_inv_latents_path,
-                               latent_store, skip_dead_source_branch)
+                               latent_store, skip_dead_source_branch, eta, generator)
         self._loop(st, self.edit_step, callback, max_steps)
         return self._output(st.latents, output_type, return_dict, decode_chunk_size)
 
     def prepare_edit(self, latents, prompt_embeds, negative_prompt_embeds, ddim_inv_prompt_embeds, image_embeddings,
                      image_latents, ddim_inv_image_embeddings, ddim_inv_image_latents, target_fps, num_inference_steps,
                      guidance_scale, ddim_init_latents_t_idx=0, ddim_inv_latents_path=None, latent_store=None,
-                     skip_dead_source_branch=True):
-        """Everything of ``sample_with_pnp`` that happens once per clip (pipeline :1014-1128)."""
+                     skip_dead_source_branch=True, eta=0.0, generator=None):
+        """Everything of ``sample_with_pnp`` that happens once per clip (pipeline :1014-1128).  ``eta > 0``: the step noise
+        is drawn from ``generator`` (one generator, or a list of one)."""
         self._guidance_scale = guidance_scale
         if not self.do_classifier_free_guidance:
             raise NotImplementedError("the PnP edit path runs with classifier-free guidance (cfg 9.0)")
+        if eta < 0:
+            raise ValueError(f"eta must be >= 0, got {eta}")
+        if eta > 0 and isinstance(generator, list) and len(generator) > 1:  # the reference's step noise would index it per frame
+            raise ValueError("eta > 0 draws the step noise from one generator: pass a single torch.Generator")
         self.check_inputs(prompt_embeds, image_latents, image_embeddings, latents)
         for name, t in (("negative_prompt_embeds", negative_prompt_embeds), ("ddim_inv_prompt_embeds", ddim_inv_prompt_embeds),
                         ("ddim_inv_image_embeddings", ddim_inv_image_embeddings), ("ddim_inv_image_latents", ddim_inv_image_latents)):
@@ -558,8 +570,8 @@ class I2VGenXLPipeline:
         cond2 = None
         if skip_dead_source_branch and not all(fires):
             cond2 = {k: v[v.shape[0] // 3:].contiguous() for k, v in cond3.items()}  # every entry is branch-major
-        st = _loop_state(latents, ts, self.scheduler, guidance_scale, dev, cond3=cond3, cond2=cond2, store=store, fires=fires,
-                         guidance=guidance_scale, skip=skip_dead_source_branch)
+        st = _loop_state(latents, ts, self.scheduler, guidance_scale, dev, eta=float(eta), cond3=cond3, cond2=cond2, store=store,
+                         fires=fires, guidance=guidance_scale, skip=skip_dead_source_branch, generator=generator)
         st.g_src = torch.zeros_like(st.latents)
         # uncond and cond are the same latents + image latents -> they share the UNet prefix up to the first cross-attention
         # (I2VGenXLUNet.forward, shared_edit_prefix); the source branch is dropped after the last injection site that fires in
@@ -593,7 +605,8 @@ class I2VGenXLPipeline:
         return None
 
     def edit_step(self, st, i: int):
-        """One iteration of the PnP edit loop (pipeline :1131-1179)."""
+        """One iteration of the PnP edit loop (pipeline :1131-1179).  With eta > 0 every step, dead-source steps included,
+        draws its noise before the UNet runs (``_draw_noise``)."""
         t = st.timesteps[i]
         register_time(self, t)
         dead_source = st.skip and not st.fires[i]
@@ -604,7 +617,8 @@ class I2VGenXLPipeline:
                 def body():
                     v = self.unet(torch.cat([st.latents, st.latents]), st.g_t, cond=st.cond2,
                                   shared_edit_prefix=st.shared_prefix)[0]
-                    st.scheduler.step(v[0:1], None, st.latents, model_output_cond=v[1:2], out=st.latents, coef_dev=st.g_coef)
+                    st.scheduler.step(v[0:1], None, st.latents, eta=st.eta, model_output_cond=v[1:2], out=st.latents,
+                                      coef_dev=st.g_coef, variance_noise=st.g_noise)
                 return body
             site = self._prune_site(flags) if st.prune_source else None
             lo = 0 if site is not None else 1  # the pruned forward returns [uncond, cond] only
@@ -612,9 +626,12 @@ class I2VGenXLPipeline:
             def body():
                 v = self.unet(torch.cat([st.g_src, st.latents, st.latents]), st.g_t, cond=st.cond3,
                               shared_edit_prefix=st.shared_prefix, prune_source_after=site)[0]
-                st.scheduler.step(v[lo:lo + 1], None, st.latents, model_output_cond=v[lo + 1:lo + 2], out=st.latents,
-                                  coef_dev=st.g_coef)
+                st.scheduler.step(v[lo:lo + 1], None, st.latents, eta=st.eta, model_output_cond=v[lo + 1:lo + 2],
+                                  out=st.latents, coef_dev=st.g_coef, variance_noise=st.g_noise)
             return body
         if not dead_source:
             st.g_src.copy_(st.store.get(t, device=st.latents.device), non_blocking=True)
-        return self._run(st, i, (dead_source, flags, self.unet.freeu_state()), make_body)
+        self._draw_noise(st)
+        # the eta = 0 keys are those of the loop without eta; eta > 0 is marked, as in call_step's key
+        key = (dead_source, flags, self.unet.freeu_state()) + ((True,) if st.eta > 0 else ())
+        return self._run(st, i, key, make_body)
