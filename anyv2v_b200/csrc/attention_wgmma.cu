@@ -8,7 +8,8 @@
 // MN-major ([keys][64], 64 contiguous) from shared memory.  With n_v = 3 (injected step) ONE P feeds the V of all three
 // branches.  K / V tiles are double-buffered with cp.async.  Rows-mode calls with 512 keys or more run attn_rows_kernel
 // instead: the same per-row algorithm, warp-specialized (TMA producer warp, mbarrier stage ring, two consumer warpgroups taking
-// turns at the tensor cores).
+// turns at the tensor cores).  av2v_tattn_fused_f16 runs tattn_fused_kernel: persistent, its Q/K/V projection fed by a TMA
+// producer through an mbarrier ring, then the same attention per item (see its comment below).
 //
 // Query slots map to token rows by mode:
 //   rows   : slot i of q tile qt -> token qt * 128 + i of sequence b; keys = the b / kv_batch_div-th key sequence.
@@ -457,67 +458,40 @@ __global__ void __launch_bounds__(kRowsThreads, 1) attn_rows_kernel(const __grid
 }
 
 // --------------------------------------------------------------------------------------------------- av2v_tattn_fused_f16
+// tattn_fused_kernel: persistent and warp-specialized.  One CTA per SM walks the items blockIdx.x, + gridDim.x, ...; items are
+// numbered heads fastest, then pixel tile, then clip, so the CTAs running at one time hold the heads of the same few pixel
+// tiles and each x tile leaves HBM once (the other heads read it from L2; the weights, 3C x Cx, stay in L2 throughout).
+// 384 threads: warpgroups 0 and 1 are the consumers (64 slots each; registers raised to 232), warpgroup 2 the producer
+// (registers lowered to 40), whose thread 0 issues the TMA loads of every projection K block of every item of the CTA into a
+// ring of tattn_stages stages.  A stage holds the x block (the item's 128 slots x 64 channels, one box of x viewed as
+// (channel, frame, pixel, clip): slot i = (pixel pix0 + i / F, frame i % F)) and the pass's weight boxes (64 x 64 rows of Q, K, V, or of V alone for the V-only passes of an n_v = 3 item).  A
+// stage has a full barrier (1 arrival + the transaction bytes) and an empty barrier (lane 0 of each of the 8 consumer warps,
+// after wgmma.wait_group has retired the MMAs that read it).  Global block g of the CTA sits in stage g % S with full phase
+// (g / S) & 1; the producer refills it after the empty phase ((g / S) - 1) & 1 (tools/kernel_models.py models this).  It runs
+// ahead across items, so the next item's first blocks land while this one runs its attention and stores.
+// Rows ppt * F .. 127 of a stage's x block (the tail, when F does not divide 128) are never written by a box of the launch,
+// all boxes having one shape: they are zeroed once, before the first load, so the tail slots project to zero Q, K, V (a
+// tail V row is multiplied by P = 0, and 0 x NaN would reach every row).  Pixels past HW are zero-filled by the TMA.
+// Per item a consumer warpgroup runs the K loop of each pass with one MMA group in flight, writes the fp16 Q / K / V of its 64
+// slots (after the other warpgroup has finished the previous item's attention: named barrier 1), and after a second barrier
+// runs the attention of its 64 slots against the keys of the same pixel and stores O.  Each accumulator sums its K blocks in
+// order, one wgmma group at a time, so results do not depend on the ring depth, the schedule or the grid size.
 struct TAttnP {
-  const __half* x;
-  const __half* wqkv;
+  CUtensorMap tx;  // x as (channel, frame, pixel, clip), box {64, F, ppt, 1}
+  CUtensorMap tw;  // wqkv [3C][Cx], box 64 x 64
   __half* o;
-  int ldx, ldo, F, HW, heads, Cx, ppt, pix_tiles, src_clips;
+  int ldo, F, HW, heads, Cx, ppt, pix_tiles, src_clips, items;
   int n_kt;  // key tiles per warpgroup: 1 (its own half) when F | 64, else 2
   float scale_log2;
 };
 
-// smem: Q, K (128 x 64 each), V per branch (128 x 64), then the projection ring: 2 stages x (A 128 x 64 + up to 3 W 64 x 64)
 template <int NV>
-constexpr int tattn_smem() { return (2 + NV) * 2 * kTile + 2 * (2 * kTile + 3 * kTile) + 1024; }
-
-// acc[part] (64 x 64 per warpgroup) = x rows of the 128 slots (xrow(slot)) @ W rows w_row0[part] .. + 64, over Cx
-template <int NP, typename XRow>
-__device__ __forceinline__ void project(const TAttnP& p, XRow xrow, const int (&w_row0)[NP], uint32_t ring, float (&acc)[NP][32]) {
-  const int wg = threadIdx.x >> 7;
-  const uint32_t stage_bytes = 2 * kTile + 3 * kTile;
-  auto load = [&](int kb, int st) {
-    const uint32_t base = ring + st * stage_bytes;
-    const int k0 = kb * 64;
-    load_tile(base, 128, p.x, [&](int r) -> const __half* {
-      const long long row = xrow(r);
-      return row < 0 ? nullptr : p.x + row * p.ldx + k0;
-    });
-#pragma unroll
-    for (int q = 0; q < NP; ++q)
-      load_tile(base + (2 + q) * kTile, 64, p.wqkv,
-                [&](int r) -> const __half* { return p.wqkv + static_cast<long long>(w_row0[q] + r) * p.Cx + k0; });
-  };
-#pragma unroll
-  for (int q = 0; q < NP; ++q)
-#pragma unroll
-    for (int i = 0; i < 32; ++i) acc[q][i] = 0.f;
-  const int nk = p.Cx / 64;
-  load(0, 0);
-  cp_async_commit();
-  for (int kb = 0; kb < nk; ++kb) {
-    if (kb + 1 < nk) {
-      load(kb + 1, (kb + 1) & 1);
-      cp_async_commit();
-      cp_async_wait<1>();
-    } else {
-      cp_async_wait<0>();
-    }
-    fence_proxy_async_smem();
-    __syncthreads();
-    const uint32_t base = ring + (kb & 1) * stage_bytes;
-    wgmma_fence();
-#pragma unroll
-    for (int q = 0; q < NP; ++q)
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        wgmma_m64n64_ss<0>(acc[q], sw128_desc(base + wg * kTile + k * 32), sw128_desc(base + (2 + q) * kTile + k * 32), 1);
-    wgmma_commit();
-    wgmma_wait<0>();
-#pragma unroll
-    for (int q = 0; q < NP; ++q) reg_fence(acc[q]);
-    __syncthreads();
-  }
-}
+__host__ __device__ constexpr int tattn_stages() { return NV == 1 ? 4 : 3; }
+constexpr int kTStageBytes = 2 * kTile + 3 * kTile;  // x block (128 x 64) + up to 3 weight boxes (64 x 64): 40 KB
+constexpr int kTThreads = 384;
+// smem: Q, K (128 x 64 each), V per branch (128 x 64), then the ring
+template <int NV>
+constexpr int tattn_smem() { return (2 + NV) * 2 * kTile + tattn_stages<NV>() * kTStageBytes + 1024; }
 
 // accumulator (64 x 64 of warpgroup wg) -> fp16 into the swizzled 128 x 64 tile at `tile` (the projection GEMM's rounding)
 __device__ __forceinline__ void acc_to_tile(const float (&acc)[32], uint32_t tile, int wg) {
@@ -530,74 +504,163 @@ __device__ __forceinline__ void acc_to_tile(const float (&acc)[32], uint32_t til
 }
 
 template <int NV>
-__global__ void __launch_bounds__(kThreads) tattn_fused_kernel(const __grid_constant__ TAttnP p) {
+__global__ void __launch_bounds__(kTThreads, 1) tattn_fused_kernel(const __grid_constant__ TAttnP p) {
+  constexpr int S = tattn_stages<NV>();
   extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t full[S], empty[S];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t sQ = smem_u32(smem), sK = sQ + 2 * kTile;
   auto sV = [&](int b) { return sQ + (2 + b) * 2 * kTile; };
   const uint32_t ring = sQ + (2 + NV) * 2 * kTile;
-  const int wg = threadIdx.x >> 7;
+  auto sX = [&](int s) { return ring + s * kTStageBytes; };
+  auto sW = [&](int s, int q) { return sX(s) + (2 + q) * kTile; };
+  const int F = p.F, C = p.heads * HD, nk = p.Cx / 64, slots = p.ppt * F;
 
-  int item = blockIdx.x;
-  const int pt = item % p.pix_tiles;
-  item /= p.pix_tiles;
-  const int h = item % p.heads;
-  const int clip = item / p.heads;  // source clip (n_v = 3) or clip
-  const int pix0 = pt * p.ppt, F = p.F, C = p.heads * HD, pix_end = min(pix0 + p.ppt, p.HW);
-  // slot i -> (pixel i / F, frame i % F) below pix_end; tail slots (i / F >= ppt) enter the projection as zero rows and are
-  // never stored
-  auto row_in = [&](int c, int i) -> long long {
-    const int pix = pix0 + i / F;
-    return pix < pix_end ? (static_cast<long long>(c) * F + i % F) * p.HW + pix : -1;
-  };
-  {
-    float acc[3][32];
-    const int w3[3] = {h * HD, C + h * HD, 2 * C + h * HD};
-    project<3>(p, [&](int i) { return row_in(clip, i); }, w3, ring, acc);
-    acc_to_tile(acc[0], sQ, wg);
-    acc_to_tile(acc[1], sK, wg);
-    acc_to_tile(acc[2], sV(0), wg);
+  {  // the tail rows of every stage's x block
+    uint8_t* ring_p = smem + (2 + NV) * 2 * kTile;
+    const int tail_chunks = (128 - slots) * 8;
+    for (int c = threadIdx.x; c < S * tail_chunks; c += kTThreads)
+      *reinterpret_cast<uint4*>(ring_p + (c / tail_chunks) * kTStageBytes + slots * 128 + (c % tail_chunks) * 16) =
+          make_uint4(0u, 0u, 0u, 0u);
+    fence_proxy_async_smem();
   }
+  if (threadIdx.x == 0) {
 #pragma unroll
-  for (int b = 1; b < NV; ++b) {
-    float acc[1][32];
-    const int w1[1] = {2 * C + h * HD};
-    project<1>(p, [&](int i) { return row_in(clip + b * p.src_clips, i); }, w1, ring, acc);
-    acc_to_tile(acc[0], sV(b), wg);
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 8);  // lane 0 of each consumer warp
+    }
+    fence_mbar_init();
   }
-  fence_proxy_async_smem();
   __syncthreads();
 
-  float o[NV][32];
+  // item -> (head h, pixel tile pt, clip): clip is the source clip at n_v = 3
+  auto decode = [&](int item, int& h, int& pix0, int& clip) {
+    h = item % p.heads;
+    item /= p.heads;
+    pix0 = item % p.pix_tiles * p.ppt;
+    clip = item / p.pix_tiles;
+  };
+
+  const int role = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 7), 0);  // warp-uniform for ptxas
+  if (role == 2) {  // ---- producer
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 256) {
+      const uint32_t x_bytes = slots * 128;
+      int g = 0;
+      for (int item = blockIdx.x; item < p.items; item += gridDim.x) {
+        int h, pix0, clip;
+        decode(item, h, pix0, clip);
+        // pass 0: Q, K, V of the (source) clip; pass b > 0: V of clip + b * src_clips
+        for (int b = 0; b < NV; ++b)
+          for (int kb = 0; kb < nk; ++kb, ++g) {
+            const int s = g % S;
+            if (g >= S) mbar_wait<false>(&empty[s], ((g / S) - 1) & 1);  // both warpgroups released block g - S
+            mbar_arrive_expect_tx(&full[s], x_bytes + (b == 0 ? 3 : 1) * kTile);
+            tma_load_4d(sX(s), &p.tx, &full[s], kb * 64, 0, pix0, clip + b * p.src_clips);
+            if (b == 0) {
 #pragma unroll
-  for (int b = 0; b < NV; ++b)
-#pragma unroll
-    for (int i = 0; i < 32; ++i) o[b][i] = 0.f;
-  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-  const int q0 = wg * 64;
-  // when F divides 64 no pixel crosses the 64-slot halves: each warpgroup then needs only its own key half.  For every other F
-  // some pixel does (e.g. F = 24: slots 48..71), so both warpgroups visit both key tiles.  The tile count is the same for both
-  // and the tile index is data, not control flow, so both issue the same wgmma sequence (no divergent path around the wgmma).
-  const int n_kt = p.n_kt;
-  for (int it = 0; it < n_kt; ++it) {
-    const int kt = n_kt == 1 ? wg : it;
-    const int k0 = kt * 64;
-    uint32_t vt[NV];
-#pragma unroll
-    for (int b = 0; b < NV; ++b) vt[b] = sV(b) + kt * kTile;
-    attn_tile<NV>(sQ + wg * kTile, sK + kt * kTile, vt, o, m, l, p.scale_log2,
-                  [&](int r, int c) { return (q0 + r) / F == (k0 + c) / F; });
+              for (int q = 0; q < 3; ++q) tma_load_4d(sW(s, q), &p.tw, &full[s], kb * 64, q * C + h * HD, 0, 0);
+            } else {
+              tma_load_4d(sW(s, 0), &p.tw, &full[s], kb * 64, 2 * C + h * HD, 0, 0);
+            }
+          }
+      }
+    }
+    return;
   }
-  // branch b writes the rows of its own clip, clip + b * src_clips
+
+  // ---- consumers
+  setmaxnreg_inc<232>();
+  const int wg = role;
+  int g = 0;  // the CTA's global K block, in the producer's order
+  // acc[q] (64 x 64 of this warpgroup's slots) = x block rows @ weight box q, over the nk K blocks of one pass
+  auto project = [&](auto& acc) {
+    constexpr int NP = sizeof(acc) / sizeof(acc[0]);
 #pragma unroll
-  for (int b = 0; b < NV; ++b) {
-    float (&ob)[1][32] = *reinterpret_cast<float(*)[1][32]>(&o[b]);
-    float lb[2] = {l[0], l[1]};
-    __half* const o1[1] = {p.o + h * HD};
-    store_o<1>(ob, lb, o1, wg, [&](int i) -> long long {
-      const long long row = row_in(clip + b * p.src_clips, i);
-      return row < 0 ? -1 : row * p.ldo;
-    });
+    for (int q = 0; q < NP; ++q)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[q][i] = 0.f;
+    for (int kb = 0; kb < nk; ++kb) {
+      const int s = (g + kb) % S;
+      mbar_wait<false>(&full[s], ((g + kb) / S) & 1);
+      wgmma_fence();
+#pragma unroll
+      for (int q = 0; q < NP; ++q)
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_m64n64_ss<0>(acc[q], sw128_desc(sX(s) + wg * kTile + k * 32), sw128_desc(sW(s, q) + k * 32), 1);
+      wgmma_commit();
+      wgmma_wait<1>();
+#pragma unroll
+      for (int q = 0; q < NP; ++q) reg_fence(acc[q]);
+      if (kb > 0) {
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[(g + kb - 1) % S]);
+      }
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int q = 0; q < NP; ++q) reg_fence(acc[q]);
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[(g + nk - 1) % S]);
+    g += nk;
+  };
+
+  const int q0 = wg * 64;
+  for (int item = blockIdx.x; item < p.items; item += gridDim.x) {
+    int h, pix0, clip;
+    decode(item, h, pix0, clip);
+    const int pix_end = min(pix0 + p.ppt, p.HW);
+    {
+      float acc[3][32];
+      project(acc);
+      // the other warpgroup has finished the previous item's attention (its reads of Q / K / V)
+      if (item != blockIdx.x) named_bar_sync(1, 256);
+      acc_to_tile(acc[0], sQ, wg);
+      acc_to_tile(acc[1], sK, wg);
+      acc_to_tile(acc[2], sV(0), wg);
+    }
+#pragma unroll
+    for (int b = 1; b < NV; ++b) {
+      float acc[1][32];
+      project(acc);
+      acc_to_tile(acc[0], sV(b), wg);
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(1, 256);
+
+    float o[NV][32];
+#pragma unroll
+    for (int b = 0; b < NV; ++b)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) o[b][i] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    // when F divides 64 no pixel crosses the 64-slot halves: each warpgroup then needs only its own key half.  For every
+    // other F some pixel does (e.g. F = 24: slots 48..71), so both warpgroups visit both key tiles.  The tile count is the
+    // same for both and the tile index is data, not control flow, so both issue the same wgmma sequence.
+    const int n_kt = p.n_kt;
+    for (int it = 0; it < n_kt; ++it) {
+      const int kt = n_kt == 1 ? wg : it;
+      const int k0 = kt * 64;
+      uint32_t vt[NV];
+#pragma unroll
+      for (int b = 0; b < NV; ++b) vt[b] = sV(b) + kt * kTile;
+      attn_tile<NV>(sQ + wg * kTile, sK + kt * kTile, vt, o, m, l, p.scale_log2,
+                    [&](int r, int c) { return (q0 + r) / F == (k0 + c) / F; });
+    }
+    // branch b writes the rows of its own clip, clip + b * src_clips; slot i holds pixel pix0 + i / F below pix_end
+#pragma unroll
+    for (int b = 0; b < NV; ++b) {
+      float (&ob)[1][32] = *reinterpret_cast<float(*)[1][32]>(&o[b]);
+      float lb[2] = {l[0], l[1]};
+      __half* const o1[1] = {p.o + h * HD};
+      const long long clip_row = static_cast<long long>(clip + b * p.src_clips) * F;
+      store_o<1>(ob, lb, o1, wg, [&](int i) -> long long {
+        const int pix = pix0 + i / F;
+        return pix < pix_end ? ((clip_row + i % F) * p.HW + pix) * p.ldo : -1;
+      });
+    }
   }
 }
 
@@ -712,10 +775,7 @@ extern "C" int av2v_tattn_fused_f16(const av2v_tattn_fused_args* a, av2v_stream_
   AV2V_REQUIRE(a->n_v == 1 || a->clips % 3 == 0, AV2V_EINVAL, "tattn_fused: n_v = 3 needs clips = 3 x clips-per-branch (got %d)", a->clips);
 
   TAttnP p{};
-  p.x = static_cast<const __half*>(a->x);
-  p.wqkv = static_cast<const __half*>(a->wqkv);
   p.o = static_cast<__half*>(a->o);
-  p.ldx = a->ldx;
   p.ldo = a->ldo;
   p.F = a->F;
   p.HW = a->HW;
@@ -728,14 +788,24 @@ extern "C" int av2v_tattn_fused_f16(const av2v_tattn_fused_args* a, av2v_stream_
   p.scale_log2 = a->scale * 1.4426950408889634f;
   const long long items = static_cast<long long>(p.src_clips) * a->heads * p.pix_tiles;
   AV2V_REQUIRE(items < (1ll << 31), AV2V_ENOSUP, "tattn_fused: too many work items");
+  p.items = static_cast<int>(items);
+  // x [clips][F][HW][ldx] as (channel, frame, pixel, clip): the box {64, F, ppt, 1} lands in slot order (pixel-major)
+  const unsigned long long row = static_cast<unsigned long long>(a->ldx) * 2, frame = row * a->HW;
+  const unsigned long long dims[4] = {static_cast<unsigned long long>(a->Cx), static_cast<unsigned long long>(a->F),
+                                      static_cast<unsigned long long>(a->HW), static_cast<unsigned long long>(a->clips)};
+  const unsigned long long strides[3] = {frame, row, frame * a->F};
+  const unsigned box[4] = {64, static_cast<unsigned>(a->F), static_cast<unsigned>(p.ppt), 1};
+  if (int e = encode_map_4d(&p.tx, a->x, dims, strides, box)) return e;
+  if (int e = encode_rows_map(&p.tw, a->wqkv, a->Cx, 3 * a->heads * HD, 1, 1, a->Cx, 0, 64)) return e;
   static bool attr_set = false;
   if (!attr_set) {
     AV2V_CHECK_CUDA(cudaFuncSetAttribute(tattn_fused_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, tattn_smem<1>()));
     AV2V_CHECK_CUDA(cudaFuncSetAttribute(tattn_fused_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, tattn_smem<3>()));
     attr_set = true;
   }
-  if (a->n_v == 3) tattn_fused_kernel<3><<<static_cast<unsigned>(items), kThreads, tattn_smem<3>(), stream>>>(p);
-  else tattn_fused_kernel<1><<<static_cast<unsigned>(items), kThreads, tattn_smem<1>(), stream>>>(p);
+  const unsigned grid = static_cast<unsigned>(items < sm_count_cached() ? items : sm_count_cached());
+  if (a->n_v == 3) tattn_fused_kernel<3><<<grid, kTThreads, tattn_smem<3>(), stream>>>(p);
+  else tattn_fused_kernel<1><<<grid, kTThreads, tattn_smem<1>(), stream>>>(p);
   AV2V_CHECK_CUDA(cudaGetLastError());
   return AV2V_OK;
 }

@@ -76,7 +76,7 @@ def simulate_gemm_ring(rng: random.Random, nk: int, stages: int, wait_depth: int
 
 # ---------------------------------------------------------------------------------------------------------- double buffer
 def simulate_double_buffer(rng: random.Random, n: int, trailing_barrier: bool = True, n_wg: int = 2):
-    """The K/V loop of attn_kernel and the projection loop of tattn_fused_kernel (project): load 0; per step kt: issue the
+    """The K/V loop of attn_kernel: load 0; per step kt: issue the
     loads of kt + 1 into buffer (kt + 1) & 1, commit, wait_group(1) (wait_group(0) on the last step) -> fence ->
     __syncthreads -> every warpgroup computes on buffer kt & 1 -> __syncthreads.  Asserts the same two hazards as the GEMM
     ring; without the trailing barrier a fast warpgroup's prefetch overwrites the buffer a slow one still reads."""
@@ -103,8 +103,8 @@ def simulate_double_buffer(rng: random.Random, n: int, trailing_barrier: bool = 
 
 def simulate_tile_handoff(rng: random.Random, barrier: bool = True, n_wg: int = 2):
     """tattn_fused_kernel between projection and attention: each warpgroup stores ITS 64 rows of the Q, K and V tiles
-    (acc_to_tile), then fence + __syncthreads, then each warpgroup's attention reads key / value rows of BOTH halves (F = 128
-    sequences span them).  Asserts every row is written before it is read."""
+    (acc_to_tile), then fence + named barrier 1 (the two consumer warpgroups), then each warpgroup's attention reads key /
+    value rows of BOTH halves (F = 128 sequences span them).  Asserts every row is written before it is read."""
     written = [rng.uniform(1, 80) for _ in range(n_wg)]  # end of each warpgroup's tile stores
     start = [w_end + rng.uniform(0, 5) for w_end in written]
     if barrier:
@@ -146,7 +146,8 @@ def frame_slot_rules():
     for rule in ("p.ppt = 128 / F;", "p.pix_tiles = (HW + p.ppt - 1) / p.ppt;", "p.f_tiles = (F + 127) / 128;",
                  "n_kv = (p.F + 63) / 64;", "const int pix_end = min(pix0 + p.ppt, p.HW);", "return pix < pix_end ?",
                  "return f < p.F ?", "return u < p.F ?", "const int nk = p.seq_kv;", "p.n_kt = 64 % a->F == 0 ? 1 : 2;",
-                 "const int kt = n_kt == 1 ? wg : it;", "C = p.heads * HD, pix_end = min(pix0 + p.ppt, p.HW);"):
+                 "const int kt = n_kt == 1 ? wg : it;", "pix0 = item % p.pix_tiles * p.ppt;",
+                 "return pix < pix_end ? ((clip_row + i % F) * p.HW + pix) * p.ldo : -1;"):
         assert rule in s, f"attention_wgmma.cu no longer contains {rule!r}"
     return True
 
@@ -698,4 +699,126 @@ def check_conv_tma_tiles(mode: str, box=None, **kw):
             kb, r, c = (int(i[0]) for i in np.nonzero(want != got))
             raise AssertionError(f"{mode} {geo}: tile row {m0} K block {kb} row {r} col {c}: TMA box holds {got[kb, r, c]}, "
                                  f"the gather {want[kb, r, c]}")
+    return True
+
+
+# ---------------------------------------------------------------------------------------------------------- persistent fused temporal attention
+def tattn_ws_constants():
+    """(stages at n_v = 1, stages at n_v = 3, empty-barrier arrivals) of tattn_fused_kernel's projection ring, as written in
+    attention_wgmma.cu; also checks the item order, block counter and parities the models below restate"""
+    s = _src("attention_wgmma.cu")
+    m = re.search(r"tattn_stages\(\) \{ return NV == 1 \? (\d+) : (\d+); \}", s)
+    k = s[s.index("tattn_fused_kernel(const"):]
+    arrivals = int(re.search(r"mbar_init\(&empty\[s\], (\d+)\);", k).group(1))
+    for rule in ("for (int item = blockIdx.x; item < p.items; item += gridDim.x)", "h = item % p.heads;",
+                 "pix0 = item % p.pix_tiles * p.ppt;", "clip = item / p.pix_tiles;",
+                 "if (g >= S) mbar_wait<false>(&empty[s], ((g / S) - 1) & 1);", "mbar_wait<false>(&full[s], ((g + kb) / S) & 1);",
+                 "mbar_arrive(&empty[(g + kb - 1) % S]);", "mbar_arrive(&empty[(g + nk - 1) % S]);",
+                 "tma_load_4d(sX(s), &p.tx, &full[s], kb * 64, 0, pix0, clip + b * p.src_clips);",
+                 "const unsigned box[4] = {64, static_cast<unsigned>(a->F), static_cast<unsigned>(p.ppt), 1};",
+                 "const unsigned long long strides[3] = {frame, row, frame * a->F};",
+                 "items < sm_count_cached() ? items : sm_count_cached()"):
+        assert rule in s, f"attention_wgmma.cu no longer contains {rule!r}: update the model"
+    return int(m.group(1)), int(m.group(2)), arrivals
+
+
+def tattn_ws_schedule(clips: int, pix_tiles: int, heads: int, sms: int):
+    """the items of each CTA (grid = min(items, sms)), decoded heads fastest.  Asserts every (clip, pixel tile, head) is run
+    once and that the items running at one time (item index // grid equal) cover whole pixel tiles: each x tile is wanted by
+    all heads at once, so it leaves HBM once"""
+    items = clips * pix_tiles * heads
+    grid = min(items, sms)
+    seen = {}
+    for b in range(grid):
+        for it in range(b, items, grid):
+            h, rest = it % heads, it // heads
+            key = (rest // pix_tiles, rest % pix_tiles, h)
+            assert key not in seen, f"item {key} run twice"
+            seen[key] = it
+    assert len(seen) == items
+    for (clip, pt, h), it in seen.items():
+        first = seen[(clip, pt, 0)]
+        assert it - first == h, f"the heads of (clip {clip}, tile {pt}) are not consecutive items"
+    return True
+
+
+def simulate_tattn_ring(rng: random.Random, n_items: int, passes: int, nk: int, stages: int, arrivals: int = 8,
+                        release: bool = True, wrong_parity: str = "", overrun: bool = False):
+    """tattn_fused_kernel's projection ring over the CTA's items.  Producer: per global block g (item, pass, kb in order), wait
+    empty[g % S] with parity ((g / S) - 1) & 1 (g >= S; skipped when overrun), then TMA into stage g % S.  Consumers w = 0, 1
+    (4 warps each): per block wait full[g % S] with parity (g / S) & 1, issue, wait_group(1) -> each warp releases block g - 1;
+    after a pass's last block wait_group(0) and release it; between items an attention phase of random length.  Asserts: no
+    block is read before it landed, no stage is refilled before both consumers released it.  Negative controls:
+    release=False (consumer 1 never releases), wrong_parity="consumer" / "producer", overrun=True."""
+    n = n_items * passes * nk
+    full = [_MBar(1) for _ in range(stages)]
+    empty = [_MBar(arrivals) for _ in range(stages)]
+    land, released = {}, {}
+    t_prod, g_prod = 0.0, 0
+    t_wg = [rng.uniform(0, 5), rng.uniform(0, 5)]
+
+    def produce_until(limit):
+        nonlocal t_prod, g_prod
+        while g_prod < min(limit, n):
+            g = g_prod
+            s = g % stages
+            if g >= stages:
+                if not overrun:
+                    if len(empty[s].done) < (g // stages) and wrong_parity != "producer":
+                        return  # the stage's release has not happened yet in this replay
+                    t_prod = empty[s].wait((((g // stages) - 1) & 1) ^ (wrong_parity == "producer"), t_prod)
+                for w in range(2):
+                    assert released.get((g - stages, w), float("inf")) <= t_prod, \
+                        f"stage {s} refilled with block {g} while block {g - stages} is read"
+            t_prod += rng.uniform(0.1, 2)
+            land[g] = t_prod + rng.uniform(5, 60)
+            full[s].arrive(land[g])
+            g_prod += 1
+
+    retire = {}
+    for g in range(n):
+        produce_until(g + stages)
+        assert g < g_prod, f"block {g} is never loaded (deadlock)"
+        kb = g % nk
+        for w in range(2):
+            t = full[g % stages].wait(((g // stages) & 1) ^ (wrong_parity == "consumer"), t_wg[w])
+            assert land[g] <= t, f"warpgroup {w} reads block {g} before it landed"
+            retire[(g, w)] = t + rng.uniform(5, 40)
+            t = max(t, retire.get((g - 1, w), 0.0)) if kb > 0 else t  # wait_group(1): block g - 1 retired
+            for b in ([g - 1] if kb > 0 else []) + ([g] if kb == nk - 1 else []):
+                if release or w == 0:
+                    done = max(t, retire[(b, w)])
+                    released[(b, w)] = done
+                    empty[b % stages].arrive(done, arrivals // 2)
+            t_wg[w] = max(t, retire[(g, w)]) if kb == nk - 1 else t
+            if kb == nk - 1 and (g // nk) % passes == passes - 1:
+                t_wg[w] += rng.uniform(10, 80)  # the item's attention and stores
+        produce_until(g + 1 + stages)
+    return True
+
+
+def tattn_box_slots(F: int, HW: int, clips: int, clip: int, pix0: int, wrong_order: bool = False):
+    """the token row each of the 128 slots of a stage's x block holds after the kernel's TMA box {64, F, ppt, 1} of x viewed as
+    (channel, frame, pixel, clip) at (0, 0, pix0, clip): box rows are written frame fastest, then pixel, so box row j is
+    (pixel pix0 + j / F, frame j % F); pixels past HW are zero-filled (-1) and the rows past ppt * F are the zeroed tail (-1).
+    wrong_order: the box walks (channel, pixel, frame), i.e. the frame and pixel strides swapped (negative control)."""
+    import numpy as np
+    ppt = 128 // F
+    slots = np.full(128, -1)
+    for j in range(ppt * F):
+        p, f = (j % ppt, j // ppt) if wrong_order else (j // F, j % F)
+        pix = pix0 + p
+        slots[j] = (clip * F + f) * HW + pix if pix < HW else -1
+    return slots
+
+
+def check_tattn_box_slots(F: int, HW: int, clips: int = 2, **kw):
+    """the box's slot contents equal frame_slot_items("fused")'s query rows for every item (tail and ragged pixels -1)"""
+    ppt = 128 // F
+    items = list(frame_slot_items("fused", F, HW, clips))
+    pix_tiles = (HW + ppt - 1) // ppt
+    for i, (qrow, _, _) in enumerate(items):
+        clip, pt = divmod(i, pix_tiles)
+        got = tattn_box_slots(F, HW, clips, clip, pt * ppt, **kw)
+        assert (got == qrow).all(), f"F={F} HW={HW} clip {clip} tile {pt}: box slots differ from the slot map"
     return True
