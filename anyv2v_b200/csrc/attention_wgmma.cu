@@ -7,9 +7,8 @@
 // registers — the accumulator layout of S is the A-fragment layout of the next wgmma — and accumulates O += P V with V read
 // MN-major ([keys][64], 64 contiguous) from shared memory.  With n_v = 3 (injected step) ONE P feeds the V of all three
 // branches.  K / V tiles are double-buffered with cp.async.  Rows-mode calls with 512 keys or more run attn_rows_kernel
-// instead: the same per-row algorithm, warp-specialized (TMA producer warp, mbarrier stage ring, two consumer warpgroups taking
-// turns at the tensor cores).  av2v_tattn_fused_f16 runs tattn_fused_kernel: persistent, its Q/K/V projection fed by a TMA
-// producer through an mbarrier ring, then the same attention per item (see its comment below).
+// instead: the same per-row algorithm, warp-specialized (ring.cuh).  av2v_tattn_fused_f16 runs tattn_fused_kernel:
+// persistent, its Q/K/V projection fed through the same ring, then the same attention per item (see its comment below).
 //
 // Query slots map to token rows by mode:
 //   rows   : slot i of q tile qt -> token qt * 128 + i of sequence b; keys = the b / kv_batch_div-th key sequence.
@@ -21,6 +20,7 @@
 //            loaded as queries nor stored, and as keys they are zero-filled and masked.
 #include "host_util.cuh"
 #include "ptx.cuh"
+#include "ring.cuh"
 
 namespace av2v {
 namespace {
@@ -257,12 +257,9 @@ constexpr int attn_smem() { return 2 * kTile + 2 * (1 + NV) * kTile + 1024; }
 // --------------------------------------------------------------------------------------------------- rows mode, pipelined
 // attn_rows_kernel: the rows-mode path of av2v_attn_pnp_f16, warp-specialized.  384 threads: warpgroup 0 is the producer (one
 // thread issues TMA loads; registers lowered to 40), warpgroups 1 and 2 are the consumers (64 query rows each; raised to 232).
-// Q (128 rows) is loaded once; K and the NV V tiles of each key tile go through a ring of kRowsStages stages, each with a
-// full mbarrier (producer arrive + TMA bytes) and an empty mbarrier (one arrive per consumer warp once the wgmma reading the
-// stage retired).  The tensor maps zero-fill keys past seq_kv and query rows past seq, so 0 * NaN never reaches PV.
-// The consumers alternate their MMA issue through named barriers 1 and 2 (ping-pong): per turn a warpgroup issues PV of tile j
-// and S = Q K^T of tile j + 1 as one wgmma group, hands the turn over, waits for the group, releases stage j and runs the
-// softmax of tile j + 1 under the other warpgroup's MMAs.
+// Q (128 rows) is loaded once; K and the NV V tiles of key tile j are ring block j (ring.cuh); the tensor maps zero-fill
+// keys past seq_kv and query rows past seq, so 0 * NaN never reaches PV.  Per turn a consumer issues PV(j) and S(j + 1)
+// as one wgmma group, hands over, waits for it, releases stage j and runs softmax(j + 1) under the other's MMAs.
 // Key tile: 128 keys at NV = 1 (S m64n128, half the rescale work of 64); 64 at NV = 3, where O alone holds 96 registers and
 // S + P of 128 keys would not fit the 168 a thread of a 384-thread CTA is compiled for.
 // Per-row algorithm as attn_tile: running max over raw scores, x = s * scale_log2 - ref in one FMA, a quarter of the
@@ -331,7 +328,8 @@ __global__ void __launch_bounds__(kRowsThreads, 1) attn_rows_kernel(const __grid
   constexpr int S = kRowsStages, KT = rows_keys<NV>(), N = KT / 2;
   constexpr uint32_t kKV = KT * 128;  // bytes of one K or V tile
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t full[S], empty[S], qbar;
+  __shared__ StageRing<S> ring;
+  __shared__ __align__(8) uint64_t qbar;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t sQ = smem_u32(smem);
   auto sK = [&](int s) { return sQ + 2 * kTile + s * (1 + NV) * kKV; };
@@ -344,11 +342,7 @@ __global__ void __launch_bounds__(kRowsThreads, 1) attn_rows_kernel(const __grid
   const int b = item / p.heads;
   const int n_kv = (p.seq_kv + KT - 1) / KT;
   if (threadIdx.x == 0) {
-#pragma unroll
-    for (int s = 0; s < S; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 8);  // lane 0 of each consumer warp
-    }
+    ring.init(8);  // every consumer warp
     mbar_init(&qbar, 1);
     fence_mbar_init();
   }
@@ -362,12 +356,11 @@ __global__ void __launch_bounds__(kRowsThreads, 1) attn_rows_kernel(const __grid
       tma_load_4d(sQ, &p.tq, &qbar, h * HD, qt * 128, b, 0);
       const int kvb = b / p.kv_div;
       for (int j = 0; j < n_kv; ++j) {
-        const int s = j % S;
-        if (j >= S) mbar_wait<false>(&empty[s], ((j / S) - 1) & 1);  // both consumers released tile j - S
-        mbar_arrive_expect_tx(&full[s], (1 + NV) * kKV);
-        tma_load_4d(sK(s), &p.tk, &full[s], h * HD, j * KT, kvb, 0);
+        const int s = ring.stage(j);
+        uint64_t* bar = ring.produce(j, (1 + NV) * kKV);
+        tma_load_4d(sK(s), &p.tk, bar, h * HD, j * KT, kvb, 0);
 #pragma unroll
-        for (int vb = 0; vb < NV; ++vb) tma_load_4d(sV(s, vb), &p.tv, &full[s], h * HD, j * KT, kvb, vb);
+        for (int vb = 0; vb < NV; ++vb) tma_load_4d(sV(s, vb), &p.tv, bar, h * HD, j * KT, kvb, vb);
       }
     }
     return;
@@ -388,65 +381,56 @@ __global__ void __launch_bounds__(kRowsThreads, 1) attn_rows_kernel(const __grid
   auto issue_s = [&](int j) {
 #pragma unroll
     for (int k = 0; k < HD / 16; ++k) {
-      if constexpr (KT == 128) wgmma_m64n128_ss(s, sw128_desc(q_wg + k * 32), sw128_desc(sK(j % S) + k * 32), k > 0);
-      else wgmma_m64n64_ss<0>(s, sw128_desc(q_wg + k * 32), sw128_desc(sK(j % S) + k * 32), k > 0);
+      if constexpr (KT == 128) wgmma_m64n128_ss(s, sw128_desc(q_wg + k * 32), sw128_desc(sK(ring.stage(j)) + k * 32), k > 0);
+      else wgmma_m64n64_ss<0>(s, sw128_desc(q_wg + k * 32), sw128_desc(sK(ring.stage(j)) + k * 32), k > 0);
     }
   };
   auto issue_pv = [&](int j) {
 #pragma unroll
     for (int vb = 0; vb < NV; ++vb)
 #pragma unroll
-      for (int kk = 0; kk < KT / 16; ++kk) wgmma_m64n64_rs<1>(o[vb], pa[kk], sw128_desc(sV(j % S, vb) + kk * 2048), 1);
+      for (int kk = 0; kk < KT / 16; ++kk) wgmma_m64n64_rs<1>(o[vb], pa[kk], sw128_desc(sV(ring.stage(j), vb) + kk * 2048), 1);
   };
   auto softmax = [&](int j) {
     const int lim = p.seq_kv - j * KT;
     if (lim >= KT) rows_softmax<NV, N, false>(s, pa, o, m, l, p.scale_log2, lim);
     else rows_softmax<NV, N, true>(s, pa, o, m, l, p.scale_log2, lim);
   };
-  // turn taking: warpgroup w waits on barrier 1 + w and hands over with an arrive on the other.  Every turn of one warpgroup
-  // is matched by one turn of the other, so warpgroup 1's arrive ahead of its first turn stands in for one after its last.
-  auto my_turn = [&] { if (wg == 0) named_bar_sync(1, 256); else named_bar_sync(2, 256); };
-  auto hand_over = [&] { if (wg == 0) named_bar_arrive(2, 256); else named_bar_arrive(1, 256); };
-  auto release = [&](int j) {
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[j % S]);
-  };
-
-  if (wg == 1) named_bar_arrive(1, 256);  // warpgroup 0 takes the first turn
+  turn_open(wg);  // both warpgroups take n_kv + 1 turns: this arrive stands in for warpgroup 1's hand-over after its last
   mbar_wait<false>(&qbar, 0);
-  mbar_wait<false>(&full[0], 0);
-  my_turn();
+  ring.wait(0);
+  turn_take(wg);
   wgmma_fence();
   issue_s(0);
   wgmma_commit();
-  hand_over();
+  turn_hand_over(wg);
   wgmma_wait<0>();
   reg_fence(s);
   softmax(0);
   for (int j = 0; j + 1 < n_kv; ++j) {
-    mbar_wait<false>(&full[(j + 1) % S], ((j + 1) / S) & 1);
-    my_turn();
+    ring.wait(j + 1);
+    turn_take(wg);
     wgmma_fence();
     issue_pv(j);
     issue_s(j + 1);
     wgmma_commit();
-    hand_over();
+    turn_hand_over(wg);
     wgmma_wait<0>();
 #pragma unroll
     for (int vb = 0; vb < NV; ++vb) reg_fence(o[vb]);
     reg_fence(s);
-    release(j);
+    ring.release(j);
     softmax(j + 1);
   }
-  my_turn();
+  turn_take(wg);
   wgmma_fence();
   issue_pv(n_kv - 1);
   wgmma_commit();
-  if (wg == 0) named_bar_arrive(2, 256);
+  if (wg == 0) turn_hand_over(wg);
   wgmma_wait<0>();
 #pragma unroll
   for (int vb = 0; vb < NV; ++vb) reg_fence(o[vb]);
-  release(n_kv - 1);
+  ring.release(n_kv - 1);
 
   __half* ob[NV];
 #pragma unroll
@@ -463,12 +447,10 @@ __global__ void __launch_bounds__(kRowsThreads, 1) attn_rows_kernel(const __grid
 // tiles and each x tile leaves HBM once (the other heads read it from L2; the weights, 3C x Cx, stay in L2 throughout).
 // 384 threads: warpgroups 0 and 1 are the consumers (64 slots each; registers raised to 232), warpgroup 2 the producer
 // (registers lowered to 40), whose thread 0 issues the TMA loads of every projection K block of every item of the CTA into a
-// ring of tattn_stages stages.  A stage holds the x block (the item's 128 slots x 64 channels, one box of x viewed as
-// (channel, frame, pixel, clip): slot i = (pixel pix0 + i / F, frame i % F)) and the pass's weight boxes (64 x 64 rows of Q, K, V, or of V alone for the V-only passes of an n_v = 3 item).  A
-// stage has a full barrier (1 arrival + the transaction bytes) and an empty barrier (lane 0 of each of the 8 consumer warps,
-// after wgmma.wait_group has retired the MMAs that read it).  Global block g of the CTA sits in stage g % S with full phase
-// (g / S) & 1; the producer refills it after the empty phase ((g / S) - 1) & 1 (tools/kernel_models.py models this).  It runs
-// ahead across items, so the next item's first blocks land while this one runs its attention and stores.
+// ring of tattn_stages stages (ring.cuh).  A stage holds the x block (the item's 128 slots x 64 channels, one box of x viewed
+// as (channel, frame, pixel, clip): slot i = (pixel pix0 + i / F, frame i % F)) and the pass's weight boxes (64 x 64 rows of
+// Q, K, V, or of V alone for the V-only passes of an n_v = 3 item).  The producer runs ahead across items, so the next item's
+// first blocks land while this one runs its attention and stores (tools/kernel_models.py models this).
 // Rows ppt * F .. 127 of a stage's x block (the tail, when F does not divide 128) are never written by a box of the launch,
 // all boxes having one shape: they are zeroed once, before the first load, so the tail slots project to zero Q, K, V (a
 // tail V row is multiplied by P = 0, and 0 x NaN would reach every row).  Pixels past HW are zero-filled by the TMA.
@@ -507,12 +489,11 @@ template <int NV>
 __global__ void __launch_bounds__(kTThreads, 1) tattn_fused_kernel(const __grid_constant__ TAttnP p) {
   constexpr int S = tattn_stages<NV>();
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t full[S], empty[S];
+  __shared__ StageRing<S> ring;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t sQ = smem_u32(smem), sK = sQ + 2 * kTile;
   auto sV = [&](int b) { return sQ + (2 + b) * 2 * kTile; };
-  const uint32_t ring = sQ + (2 + NV) * 2 * kTile;
-  auto sX = [&](int s) { return ring + s * kTStageBytes; };
+  auto sX = [&](int s) { return sQ + (2 + NV) * 2 * kTile + s * kTStageBytes; };  // the stages follow V
   auto sW = [&](int s, int q) { return sX(s) + (2 + q) * kTile; };
   const int F = p.F, C = p.heads * HD, nk = p.Cx / 64, slots = p.ppt * F;
 
@@ -525,11 +506,7 @@ __global__ void __launch_bounds__(kTThreads, 1) tattn_fused_kernel(const __grid_
     fence_proxy_async_smem();
   }
   if (threadIdx.x == 0) {
-#pragma unroll
-    for (int s = 0; s < S; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 8);  // lane 0 of each consumer warp
-    }
+    ring.init(8);  // every consumer warp
     fence_mbar_init();
   }
   __syncthreads();
@@ -554,15 +531,14 @@ __global__ void __launch_bounds__(kTThreads, 1) tattn_fused_kernel(const __grid_
         // pass 0: Q, K, V of the (source) clip; pass b > 0: V of clip + b * src_clips
         for (int b = 0; b < NV; ++b)
           for (int kb = 0; kb < nk; ++kb, ++g) {
-            const int s = g % S;
-            if (g >= S) mbar_wait<false>(&empty[s], ((g / S) - 1) & 1);  // both warpgroups released block g - S
-            mbar_arrive_expect_tx(&full[s], x_bytes + (b == 0 ? 3 : 1) * kTile);
-            tma_load_4d(sX(s), &p.tx, &full[s], kb * 64, 0, pix0, clip + b * p.src_clips);
+            const int s = ring.stage(g);
+            uint64_t* bar = ring.produce(g, x_bytes + (b == 0 ? 3 : 1) * kTile);
+            tma_load_4d(sX(s), &p.tx, bar, kb * 64, 0, pix0, clip + b * p.src_clips);
             if (b == 0) {
 #pragma unroll
-              for (int q = 0; q < 3; ++q) tma_load_4d(sW(s, q), &p.tw, &full[s], kb * 64, q * C + h * HD, 0, 0);
+              for (int q = 0; q < 3; ++q) tma_load_4d(sW(s, q), &p.tw, bar, kb * 64, q * C + h * HD, 0, 0);
             } else {
-              tma_load_4d(sW(s, 0), &p.tw, &full[s], kb * 64, 2 * C + h * HD, 0, 0);
+              tma_load_4d(sW(s, 0), &p.tw, bar, kb * 64, 2 * C + h * HD, 0, 0);
             }
           }
       }
@@ -582,8 +558,8 @@ __global__ void __launch_bounds__(kTThreads, 1) tattn_fused_kernel(const __grid_
 #pragma unroll
       for (int i = 0; i < 32; ++i) acc[q][i] = 0.f;
     for (int kb = 0; kb < nk; ++kb) {
-      const int s = (g + kb) % S;
-      mbar_wait<false>(&full[s], ((g + kb) / S) & 1);
+      const int s = ring.stage(g + kb);
+      ring.wait(g + kb);
       wgmma_fence();
 #pragma unroll
       for (int q = 0; q < NP; ++q)
@@ -594,16 +570,12 @@ __global__ void __launch_bounds__(kTThreads, 1) tattn_fused_kernel(const __grid_
       wgmma_wait<1>();
 #pragma unroll
       for (int q = 0; q < NP; ++q) reg_fence(acc[q]);
-      if (kb > 0) {
-        __syncwarp();
-        if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[(g + kb - 1) % S]);
-      }
+      if (kb > 0) ring.release(g + kb - 1);
     }
     wgmma_wait<0>();
 #pragma unroll
     for (int q = 0; q < NP; ++q) reg_fence(acc[q]);
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[(g + nk - 1) % S]);
+    ring.release(g + nk - 1);
     g += nk;
   };
 

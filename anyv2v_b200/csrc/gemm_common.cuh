@@ -1,6 +1,6 @@
 // Shared by the two GEMM kernels: the launch parameters av2v_gemm_f16 validates and fills, the GEGLU activation and the
 // staged epilogue.
-//   gemm_linear_ws.cu  : persistent and warp-specialized, TMA-fed: the LINEAR mode, and the conv modes (3 x 3 stride 1, up2
+//   gemm_ws.cu         : persistent and warp-specialized, TMA-fed: the LINEAR mode, and the conv modes (3 x 3 stride 1, up2
 //                        phase, temporal (3, 1, 1)) whose 128-row tiles are each one box of the input (conv_ws_box)
 //   gemm_wgmma.cu      : the other conv geometries (stride 2, widths that do not divide 128, ...), cp.async-gathered, two
 //                        CTAs per SM
@@ -158,7 +158,7 @@ __device__ __forceinline__ void copy_out_band(const GemmP& p, int slot, int m0, 
   }
 }
 
-// Launches of gemm_linear_ws.cu's persistent kernel on `tiles` output tiles; p is validated and filled by av2v_gemm_f16.
+// Launches of gemm_ws.cu's persistent kernel on `tiles` output tiles; p is validated and filled by av2v_gemm_f16.
 // LINEAR mode; a conv mode whose tiles are each one box of its input (conv_ws_box returns true and the box).
 int gemm_linear_ws(const GemmP& p, int tiles, cudaStream_t stream);
 bool conv_ws_box(const GemmP& p, unsigned (&box)[3]);

@@ -1,7 +1,7 @@
-// wgmma GEMM core of the I2VGen-XL UNet hot path (sm_90a): the convolutions gemm_linear_ws.cu's persistent kernel does not
+// wgmma GEMM core of the I2VGen-XL UNet hot path (sm_90a): the convolutions gemm_ws.cu's persistent kernel does not
 // take.  av2v_gemm_f16 validates every call the same way whichever kernel runs it, then sends the LINEAR mode, and every
 // conv whose 128-row tiles are each one TMA box of its input (conv_ws_box: 3 x 3 stride 1 and up2 phases at widths that
-// divide 128, temporal convs whose tiles hold whole frames of one clip), to gemm_linear_ws.cu; the rest (stride 2, widths
+// divide 128, temporal convs whose tiles hold whole frames of one clip), to gemm_ws.cu; the rest (stride 2, widths
 // such as 27 or 88, temporal convs whose frame count the box does not divide) run here.
 //
 //   out[slot][m, n] = sum_k A[m, k] * W[n, k] + bias[n] + rowbias[m / rows_per_rowbias, n] + residual[slot][m, n]

@@ -265,7 +265,7 @@ class _GEGLU(nn.Module):
 
     def packed(self):
         """(weight, bias) with the h / gate halves interleaved in blocks of 32 rows: the layout of the fused GEGLU
-        epilogue (csrc/gemm_linear_ws.cu), which stores h * gelu_erf(gate) and never materialises the [rows, 8C] tensor."""
+        epilogue (csrc/gemm_ws.cu), which stores h * gelu_erf(gate) and never materialises the [rows, 8C] tensor."""
         w = self.proj.weight
         key = (w.data_ptr(), w._version, self.proj.bias.data_ptr(), self.proj.bias._version)
         if self._packed._key != key:

@@ -1,4 +1,4 @@
-"""CPU tests of the conv A operand of the persistent GEMM kernel (csrc/gemm_linear_ws.cu, gemm_ws_kernel<true>), through the
+"""CPU tests of the conv A operand of the persistent GEMM kernel (csrc/gemm_ws.cu, gemm_ws_kernel<true>), through the
 model of tools/kernel_models.py: per output tile and K block, the TMA box the producer loads (its origin, the tap walk and
 TMA's zero-fill outside the tensor) holds element for element what gemm_wgmma_kernel's cp.async gather loads; and the
 dispatch rule (conv_ws_box) sends the UNet's geometries where a box exists, the others to gemm_wgmma_kernel.  Negative

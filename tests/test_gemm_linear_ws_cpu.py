@@ -1,4 +1,4 @@
-"""CPU tests of the model of gemm_linear_ws_kernel's schedule (tools/kernel_models.py: linear_ws_schedule, simulate_linear_ws):
+"""CPU tests of the model of gemm_ws_kernel's schedule (tools/kernel_models.py: linear_ws_schedule, simulate_linear_ws):
 the persistent tile schedule, the TMA stage ring across tile boundaries, the consumers' turn taking and the reuse of each
 staging tile, each with a negative control."""
 import os

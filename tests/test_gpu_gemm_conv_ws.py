@@ -1,4 +1,4 @@
-"""GPU tests of the conv modes on the persistent, TMA-fed GEMM kernel (csrc/gemm_linear_ws.cu, gemm_ws_kernel<true>) against
+"""GPU tests of the conv modes on the persistent, TMA-fed GEMM kernel (csrc/gemm_ws.cu, gemm_ws_kernel<true>) against
 the float64 contracts of tests/kernel_contracts.py, within ulp16(ref) + kappa * cond (tests/ulp_check.py), on guarded
 buffers (tests/guarded.py).
 

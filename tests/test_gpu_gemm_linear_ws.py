@@ -1,4 +1,4 @@
-"""GPU tests of the LINEAR-mode GEMM (csrc/gemm_linear_ws.cu, persistent and warp-specialized) against the float64 contract
+"""GPU tests of the LINEAR-mode GEMM (csrc/gemm_ws.cu, persistent and warp-specialized) against the float64 contract
 of tests/kernel_contracts.py, within ulp16(ref) + kappa * cond (tests/ulp_check.py), on guarded buffers (tests/guarded.py).
 
 The kernel runs min(tiles, SMs) CTAs that walk a static tile schedule, two consumer warpgroups taking turns per tile, and

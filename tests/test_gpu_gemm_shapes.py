@@ -1,4 +1,4 @@
-"""GPU tests of the GEMM (csrc/gemm_wgmma.cu: the conv modes, csrc/gemm_linear_ws.cu: LINEAR) against the float64
+"""GPU tests of the GEMM (csrc/gemm_wgmma.cu: the conv modes, csrc/gemm_ws.cu: LINEAR) against the float64
 contracts of tests/kernel_contracts.py, within ulp16(ref) + kappa * cond (tests/ulp_check.py), on guarded buffers
 (tests/guarded.py).
 

@@ -15,9 +15,11 @@ heads) and transformer_in (HW 4096, Cx 320, 8 heads), at n_v = 1 (one clip) and 
 Beside each, the unfused control times the same computation as the UNet's other path does it: ops.linear for Q|K|V (Q|K of
 the source clip and V of all three at n_v = 3) and the frames-mode ops.attention.  Their FLOPs count only the slots that
 hold a frame, not the empty tail of a CTA's 128 slots: the projections (2 * Cx * 64 per head and row, for Q and K of the
-source rows and V of every row) plus QK^T and PV over the F frames of each pixel.  The fused kernel's outputs of every build
-are compared with this build's (torch.equal), and its x-read rate (bytes of x over the call time) is printed: a kernel that
-reads x from HBM once per call is bounded by it at 3.35 TB/s.  A build that rejects a case is reported as "unsupported"."""
+source rows and V of every row) plus QK^T and PV over the F frames of each pixel.  The fused kernel's x-read rate (bytes of x
+over the call time) is printed: a kernel that reads x from HBM once per call is bounded by it at 3.35 TB/s.
+
+The outputs of every build are compared with this build's (torch.equal) for the rows-mode cases (attn_rows_kernel at 512 keys
+or more, attn_kernel below) and the fused ones.  A build that rejects a case is reported as "unsupported"."""
 from __future__ import annotations
 
 import argparse
@@ -77,7 +79,7 @@ def _fused_cases(dev, frames):
 
 
 def _cases(dev):
-    """name -> (fn, flops)"""
+    """name -> (fn, flops, out, 0); out: the rows every case of a level writes, o[:B * seq] (n_v = 3: 3 branches of B / 3)"""
     torch.manual_seed(0)
     cases = {}
     for step, B in (("inv", 16), ("edit", 48)):
@@ -88,19 +90,19 @@ def _cases(dev):
             o = torch.empty(3 * B * seq, C, device=dev).half()
             cases[f"{step} self   {seq:4d}x{heads:2d} b{B} nv1"] = (
                 lambda q=q, kv=kv, o=o, h=heads, s=seq, b=B, C=C: ops.attention(q, kv[:, :C], kv[:, C:], h, s, b, o[:b * s]),
-                4 * B * heads * seq * seq * 64, None, 0)
+                4 * B * heads * seq * seq * 64, o[:B * seq], 0)
             if step == "edit":  # injected: Q / K of the 16 source sequences, V of all three branches
                 S = B // 3
                 cases[f"{step} inject {seq:4d}x{heads:2d} b{S} nv3"] = (
                     lambda q=q, kv=kv, o=o, h=heads, s=seq, S=S, C=C: ops.attention(
                         q[:S * s], kv[:S * s, :C], kv[:, C:], h, s, S, o, n_v=3, v_branch_stride=S * s * 2 * C,
                         o_branch_stride=S * s * C),
-                    2 * (1 + 3) * S * heads * seq * seq * 64, None, 0)
+                    2 * (1 + 3) * S * heads * seq * seq * 64, o[:B * seq], 0)
             ctx = torch.randn(B // 16 * N_CTX, 2 * C, device=dev).half()
             cases[f"{step} cross  {seq:4d}x{heads:2d} b{B} kv{N_CTX}"] = (
                 lambda q=q, ctx=ctx, o=o, h=heads, s=seq, b=B, C=C: ops.attention(
                     q, ctx[:, :C], ctx[:, C:], h, s, b, o[:b * s], seq_kv=N_CTX, kv_batch_div=16),
-                4 * B * heads * seq * N_CTX * 64, None, 0)
+                4 * B * heads * seq * N_CTX * 64, o[:B * seq], 0)
     return cases
 
 
@@ -120,7 +122,7 @@ def main():
     times = {(lib, c): [] for lib in libs for c in cases}
     unsupported = set()
     outs = {}
-    for name, lib in libs.items():  # warm-up: module load, first launches; the fused kernel's outputs of each build
+    for name, lib in libs.items():  # warm-up: module load, first launches; the outputs of each build
         _lib._lib = lib
         for c, (fn, _, out, _) in cases.items():
             try:

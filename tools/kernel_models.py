@@ -1,5 +1,5 @@
-"""CPU models of the synchronisation and index bookkeeping of the sm_90a kernels (csrc/gemm_wgmma.cu, csrc/gemm_linear_ws.cu,
-csrc/gemm_common.cuh, csrc/attention_wgmma.cu).
+"""CPU models of the synchronisation and index bookkeeping of the sm_90a kernels (csrc/gemm_wgmma.cu, csrc/gemm_ws.cu,
+csrc/gemm_common.cuh, csrc/attention_wgmma.cu, csrc/ring.cuh).
 
 A data race or a wrong index in these kernels shows up on the GPU only as occasionally wrong numbers, so the schedules are
 restated here as discrete-event models with randomised latencies and checked for their hazards, each with a negative control
@@ -254,9 +254,9 @@ def check_epilogue_staging(kernel: str, geglu: bool = False, swizzle: bool = Tru
     src = _src("gemm_common.cuh")
     assert "return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));" in src, "stage_offset changed: update the model"
     for f, rule in (("gemm_wgmma.cu", "const int r0 = 16 * (threadIdx.x >> 5);"),
-                    ("gemm_linear_ws.cu", "const int r0 = 16 * ((threadIdx.x >> 5) & 3);"),
-                    ("gemm_linear_ws.cu", "fetch_residual_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);"),
-                    ("gemm_linear_ws.cu", "copy_out_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);")):
+                    ("gemm_ws.cu", "const int r0 = 16 * ((threadIdx.x >> 5) & 3);"),
+                    ("gemm_ws.cu", "fetch_residual_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);"),
+                    ("gemm_ws.cu", "copy_out_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);")):
         assert rule in _src(f), f"{f} no longer contains {rule!r}: update the model"
     bands = epilogue_bands(kernel)
     lg = 3 if geglu else 4  # log2(chunks per tile row): the GEGLU output tile is 128 x 64
@@ -350,16 +350,29 @@ def check_epilogue(geglu_pack, N_geglu=(128, 256, 2560)):
     return True
 
 
-# ---------------------------------------------------------------------------------------------------------- rows attention ring
-def rows_ring_constants():
-    """(stages, empty-barrier arrivals) of attn_rows_kernel's K / V ring, as written in attention_wgmma.cu; also checks that the
-    producer and consumer waits use the parities the model assumes"""
-    s = _src("attention_wgmma.cu")
-    stages = int(re.search(r"constexpr int kRowsStages = (\d+);", s).group(1))
-    arrivals = int(re.search(r"mbar_init\(&empty\[s\], (\d+)\);", s).group(1))
-    assert "mbar_wait<false>(&empty[s], ((j / S) - 1) & 1)" in s
-    assert "mbar_wait<false>(&full[(j + 1) % S], ((j + 1) / S) & 1)" in s and "mbar_wait<false>(&full[0], 0)" in s
-    return stages, arrivals
+# ---------------------------------------------------------------------------------------------------------- stage ring
+def kernel_body(name, kernel):
+    """the source text of __global__ `kernel` in csrc/`name`, from its name to its closing brace"""
+    s = _src(name)
+    i = s.index(f" {kernel}(const __grid_constant__")
+    return s[i:s.index("\n}\n", i)]
+
+
+def ring_constants():
+    """StageRing's rules as ring.cuh writes them, each a function of (g, S): the stage of block g, the full parity its consumer
+    waits on, whether producing it waits on empty (refill) and on which parity; also checks the arrival counts RingModel
+    assumes (full: 1, empty: one per consumer warp, released by lane 0 after __syncwarp)"""
+    s = _src("ring.cuh")
+    for rule in ("mbar_init(&full[s], 1);", "mbar_init(&empty[s], consumer_warps);",
+                 "__syncwarp();\n    if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[stage(g)]);"):
+        assert rule in s, f"ring.cuh no longer contains {rule!r}: update the model"
+
+    def rule(pattern):
+        return eval("lambda g, S: " + re.search(pattern, s).group(1).replace("/", "//"))  # C division of g >= 0
+    return dict(stage=rule(r"int stage\(int g\) \{ return (.+?); \}"),
+                full=rule(r"mbar_wait<false>\(&full\[stage\(g\)\], (.+?)\);"),
+                refill=rule(r"if \((.+?)\) mbar_wait<false>\(&empty"),
+                empty=rule(r"mbar_wait<false>\(&empty\[stage\(g\)\], (.+?)\);"))
 
 
 class _MBar:
@@ -381,51 +394,86 @@ class _MBar:
         raise AssertionError(f"wait on parity {parity} never succeeds (deadlock)")
 
 
-def simulate_rows_ring(rng: random.Random, n: int, stages: int, arrivals: int = 8, release: bool = True,
-                       wrong_parity: str = "", pingpong: bool = True):
-    """attn_rows_kernel's schedule.  Producer: per tile j, wait empty[j % S] with parity ((j / S) - 1) & 1 (j >= S), arrive +
-    TMA into stage j % S (full completes when the bytes land).  Consumers w = 0, 1 (4 warps each): turn 0 issues S(0); turn
-    k = 1 .. n issues PV(k - 1) and S(k) (k < n) after waiting full[k % S] with parity (k / S) & 1; turns alternate through the
-    named barriers (w = 0 first); after the wgmma group retired, each warp arrives on empty[(k - 1) % S].  Asserts: no tile is
-    read before it landed, no stage is refilled before both consumers released it, the MMA turns alternate 0, 1, 0, 1, ...
-    Negative controls: release=False (consumer 1 never releases), wrong_parity="consumer" / "producer", pingpong=False."""
-    full = [_MBar(1) for _ in range(stages)]
-    empty = [_MBar(arrivals) for _ in range(stages)]
-    land, released, turns = {}, {}, []
-    t_prod = 0.0
+class RingModel:
+    """StageRing<stages> (ring.cuh) under randomised TMA latencies, with the rules ring_constants() reads.  The producer thread
+    is replayed on demand and in block order (wait(g) first produces every block up to g); its times depend only on its own
+    empty waits and issue, so it runs ahead as the kernel's does.  Each block is read and released by `readers` consumer
+    warpgroups of arrivals / readers warps (2 in the attention kernels; 1 in the GEMM, where a tile belongs to one).
+    Asserts: no block is read before it landed, no stage is refilled before every reader released the block it held.
+    Faults (negative controls): wrong_parity="producer" / "consumer" flips that side's wait parity, release=False (one warp
+    of warpgroup 1 never arrives on empty), overrun (the producer skips its empty wait)."""
+    def __init__(self, rng, stages, arrivals, readers, wrong_parity="", release=True, overrun=False):
+        self.rng, self.S, self.readers, self.warps = rng, stages, readers, arrivals // readers
+        self.rules = ring_constants()
+        self.full = [_MBar(1) for _ in range(stages)]
+        self.empty = [_MBar(arrivals) for _ in range(stages)]
+        self.flip = {side: int(wrong_parity == side) for side in ("producer", "consumer")}
+        self.release_ok, self.overrun = release, overrun
+        self.land, self.released = {}, {}  # block -> landing time; block -> release times of its readers
+        self.t_prod = 0.0
+
+    def _produce(self, g):
+        r, S = self.rules, self.S
+        s = r["stage"](g, S)
+        if r["refill"](g, S):
+            if not self.overrun:
+                self.t_prod = self.empty[s].wait(r["empty"](g, S) ^ self.flip["producer"], self.t_prod)
+            done = self.released.get(g - S, [])
+            assert len(done) == self.readers and max(done) <= self.t_prod, \
+                f"stage {s} refilled with block {g} while block {g - S} is read"
+        self.t_prod += self.rng.uniform(0.1, 2)
+        self.land[g] = self.t_prod + self.rng.uniform(5, 60)
+        self.full[s].arrive(self.land[g])
+
+    def wait(self, g, w, t):
+        """warpgroup w, at time t, waits for block g; returns when it may read it"""
+        while len(self.land) <= g:
+            self._produce(len(self.land))
+        t = self.full[self.rules["stage"](g, self.S)].wait(self.rules["full"](g, self.S) ^ self.flip["consumer"], t)
+        assert self.land[g] <= t, f"warpgroup {w} reads block {g} before it landed"
+        return t
+
+    def release(self, g, w, t):
+        """every warp of warpgroup w releases block g at time t"""
+        short = not self.release_ok and w == 1
+        self.empty[self.rules["stage"](g, self.S)].arrive(t, self.warps - short)
+        if not short:
+            self.released.setdefault(g, []).append(t)
+
+
+# ---------------------------------------------------------------------------------------------------------- rows attention ring
+def rows_ring_constants():
+    """(stages, empty-barrier arrivals) of attn_rows_kernel's K / V ring, as written in attention_wgmma.cu; also checks the
+    tile order and turn closing the model restates"""
+    k = kernel_body("attention_wgmma.cu", "attn_rows_kernel")
+    stages = int(re.search(r"constexpr int kRowsStages = (\d+);", _src("attention_wgmma.cu")).group(1))
+    arrivals = int(re.search(r"ring\.init\((\d+)\);", k).group(1))
+    for rule in ("constexpr int S = kRowsStages,", "for (int j = 0; j < n_kv; ++j) {", "ring.produce(j, ", "ring.wait(0);",
+                 "ring.wait(j + 1);", "ring.release(j);", "ring.release(n_kv - 1);", "if (wg == 0) turn_hand_over(wg);"):
+        assert rule in k, f"attn_rows_kernel no longer contains {rule!r}: update the model"
+    return stages, arrivals
+
+
+def simulate_rows_ring(rng: random.Random, n: int, stages: int, arrivals: int = 8, pingpong: bool = True, **faults):
+    """attn_rows_kernel's consumers w = 0, 1 on the ring (RingModel, tile j = block j): turn 0 issues S(0); turn k = 1 .. n
+    issues PV(k - 1) and S(k) (k < n, after waiting for tile k); turns alternate through the named barriers (w = 0 first);
+    once the wgmma group retired the warpgroup releases tile k - 1 and runs the softmax of tile k.  Asserts, beside the
+    ring's: the MMA turns alternate 0, 1, 0, 1, ...  Negative controls: RingModel's faults, pingpong=False."""
+    ring = RingModel(rng, stages, arrivals, 2, **faults)
+    turns = []
     t_wg = [rng.uniform(0, 5), rng.uniform(0, 5)]
     handed = [0.0, None]  # handed[w]: when the other warpgroup last handed the turn to w (w = 0 starts with it)
-
-    def produce(j):
-        nonlocal t_prod
-        s = j % stages
-        if j >= stages:
-            par = ((j // stages) - 1) & 1
-            t_prod = empty[s].wait(par ^ (wrong_parity == "producer"), t_prod)
-            for w in range(2):
-                assert released[(j - stages, w)] <= t_prod, f"stage {s} refilled with tile {j} while tile {j - stages} is read"
-        t_prod += rng.uniform(0.1, 2)
-        land[j] = t_prod + rng.uniform(5, 60)
-        full[s].arrive(land[j])
-
     for k in range(n + 1):
-        if k < n:
-            produce(k)
         for w in range(2):
-            t = t_wg[w]
-            if k < n:
-                t = full[k % stages].wait(((k // stages) & 1) ^ (wrong_parity == "consumer"), t)
+            t = ring.wait(k, w, t_wg[w]) if k < n else t_wg[w]
             if pingpong:
                 assert handed[w] is not None
                 t = max(t, handed[w])
-            for tile in ([k] if k < n else []) + ([k - 1] if k > 0 else []):
-                assert land[tile] <= t, f"warpgroup {w} reads tile {tile} before it landed"
             turns.append((t, w))
             handed[1 - w] = t + rng.uniform(0.1, 1)
             retire = t + rng.uniform(5, 40)
-            if k > 0 and (release or w == 0):
-                released[(k - 1, w)] = retire
-                empty[(k - 1) % stages].arrive(retire, arrivals // 2)
+            if k > 0:
+                ring.release(k - 1, w, retire)
             t_wg[w] = retire + rng.uniform(1, 30)  # softmax of tile k
     order = [w for _, w in sorted(turns, key=lambda x: x[0])]
     assert order == [0, 1] * (n + 1), "MMA turns of the two consumers do not alternate"
@@ -434,18 +482,19 @@ def simulate_rows_ring(rng: random.Random, n: int, stages: int, arrivals: int = 
 
 # ---------------------------------------------------------------------------------------------------------- persistent LINEAR GEMM
 def linear_ws_constants():
-    """(stages, empty-barrier arrivals) of gemm_ws_kernel's ring, as written in gemm_linear_ws.cu; also checks that the
-    tile schedule, the barrier parities and the turn taking are the ones the models below restate"""
-    s = _src("gemm_linear_ws.cu")
-    stages = int(re.search(r"constexpr int kStages = (\d+);", s).group(1))
-    arrivals = int(re.search(r"mbar_init\(&empty\[s\], (\d+)\);", s).group(1))
-    for rule in ("for (int t = blockIdx.x; t < P.tiles; t += gridDim.x)",
+    """(stages, empty-barrier arrivals) of gemm_ws_kernel's ring, as written in gemm_ws.cu; also checks that the tile
+    schedule, the block numbering and the turn taking are the ones the models below restate"""
+    k = kernel_body("gemm_ws.cu", "gemm_ws_kernel")
+    stages = int(re.search(r"constexpr int kStages = (\d+);", _src("gemm_ws.cu")).group(1))
+    arrivals = int(re.search(r"ring\.init\((\d+)\);", k).group(1))
+    for rule in ("StageRing<kStages> ring;", "for (int t = blockIdx.x; t < P.tiles; t += gridDim.x)",
+                 "for (int kb = 0; kb < nk; ++kb, ++g) {", "ring.produce(g, kStageBytes);",
                  "for (int i = wg, t = blockIdx.x + wg * gridDim.x; t < P.tiles; i += 2, t += 2 * gridDim.x)",
-                 "const int g0 = i * nk;", "const int s = g % kStages, k0 = kb * BK;",
-                 "mbar_wait<false>(&empty[s], ((g / kStages) - 1) & 1)", "mbar_wait<false>(&full[s], (g / kStages) & 1)",
-                 "if (kb > 0) release(g - 1);", "release(g0 + nk - 1);", "if (wg == 1) named_bar_arrive(1, 256);",
-                 "if (t + gridDim.x < P.tiles) hand_over();", "tiles < sm_count_cached() ? tiles : sm_count_cached()"):
-        assert rule in s, f"gemm_linear_ws.cu no longer contains {rule!r}: update the model"
+                 "const int g0 = i * nk;", "const int g = g0 + kb, s = ring.stage(g);", "ring.wait(g);",
+                 "if (kb > 0) ring.release(g - 1);", "ring.release(g0 + nk - 1);", "turn_open(wg);",
+                 "if (t + gridDim.x < P.tiles) turn_hand_over(wg);"):
+        assert rule in k, f"gemm_ws_kernel no longer contains {rule!r}: update the model"
+    assert "tiles < sm_count_cached() ? tiles : sm_count_cached()" in _src("gemm_ws.cu")
     return stages, arrivals
 
 
@@ -469,47 +518,22 @@ def linear_ws_schedule(tiles: int, sms: int, off_by_one: bool = False):
     return True
 
 
-def simulate_linear_ws(rng: random.Random, n_tiles: int, nk: int, stages: int, arrivals: int = 4, release: bool = True,
-                       wrong_parity: str = "", pingpong: bool = True, early_refill: bool = False):
-    """one CTA of gemm_ws_kernel with n_tiles tiles of nk K blocks.  Producer: block g = i * nk + kb in stage g % S,
-    waits empty with parity ((g / S) - 1) & 1 (g >= S), then TMA (full completes when the bytes land).  Consumer w takes local
-    tiles i = w, w + 2, ...: fetches the tile's residual into its staging tile (cp.async), waits for its turn (warpgroup 1
-    arrives on warpgroup 0's barrier first; a warpgroup hands over after issuing its last MMA when a tile follows), per block
-    waits full with parity (g / S) & 1, issues, and releases block g - 1 once wgmma.wait_group(1) retired it (the last block
-    after wait_group(0)); then the epilogue and the copy-out of the staging tile.  Asserts: no block read before it landed, no
-    stage refilled before its block was released by every consumer warp, the K loops run one at a time in order 0, 1, 0, 1
-    ..., and a staging tile is refilled only after its copy-out read it.  Negative controls: release=False (a warp never
-    arrives on empty), wrong_parity="producer" / "consumer", pingpong=False, early_refill (the next residual fetch issued
-    before the copy-out)."""
-    full = [_MBar(1) for _ in range(stages)]
-    empty = [_MBar(arrivals) for _ in range(stages)]
-    land, released, loops = {}, {}, []
-    t_prod = 0.0
+def simulate_linear_ws(rng: random.Random, n_tiles: int, nk: int, stages: int, arrivals: int = 4, pingpong: bool = True,
+                       early_refill: bool = False, **faults):
+    """one CTA of gemm_ws_kernel with n_tiles tiles of nk K blocks on the ring (RingModel, block g = i * nk + kb, read by the
+    tile's warpgroup alone).  Consumer w takes local tiles i = w, w + 2, ...: fetches the tile's residual into its staging
+    tile (cp.async), waits for its turn (warpgroup 1 arrives on warpgroup 0's barrier first; a warpgroup hands over after
+    issuing its last MMA when a tile follows), per block waits for it, issues, and releases block g - 1 once
+    wgmma.wait_group(1) retired it (the last block after wait_group(0)); then the epilogue and the copy-out of the staging
+    tile.  Asserts, beside the ring's: the K loops run one at a time in order 0, 1, 0, 1 ..., and a staging tile is refilled
+    only after its copy-out read it.  Negative controls: RingModel's faults, pingpong=False, early_refill (the next residual
+    fetch issued before the copy-out)."""
+    ring = RingModel(rng, stages, arrivals, 1, **faults)
+    loops = []
     t_wg = [rng.uniform(0, 5), rng.uniform(0, 5)]
     handed = [rng.uniform(0, 1), None]  # handed[w]: when the turn was handed to w (warpgroup 1's opening arrive: tile 0)
     copy_done = [None, None]      # end of the last copy-out of each staging tile
     next_fetch = [None, None]     # early_refill: when the next tile's fetch was issued
-    produced = 0
-
-    def produce_until(g_max):
-        nonlocal t_prod, produced
-        while produced <= g_max and produced < n_tiles * nk:
-            g, s = produced, produced % stages
-            if g >= stages:
-                par = ((g // stages) - 1) & 1
-                t_prod = empty[s].wait(par ^ (wrong_parity == "producer"), t_prod)
-                assert released.get(g - stages, float("inf")) <= t_prod, f"stage {s} refilled with block {g} while block {g - stages} is read"
-            t_prod += rng.uniform(0.1, 2)
-            land[g] = t_prod + rng.uniform(5, 60)
-            full[s].arrive(land[g])
-            produced += 1
-
-    def release_block(g, t):
-        n = arrivals if release else arrivals - 1
-        empty[g % stages].arrive(t, n)
-        if release:
-            released[g] = t
-
     for i in range(n_tiles):
         w = i % 2
         t = t_wg[w]
@@ -525,27 +549,24 @@ def simulate_linear_ws(rng: random.Random, n_tiles: int, nk: int, stages: int, a
         prev_retire = 0.0
         for kb in range(nk):
             g = i * nk + kb
-            produce_until(g)
-            t = full[g % stages].wait(((g // stages) & 1) ^ (wrong_parity == "consumer"), t)
-            assert land[g] <= t, f"warpgroup {w} reads block {g} before it landed"
+            t = ring.wait(g, w, t)
             t += rng.uniform(0.1, 2)                     # issue
             retire = t + rng.uniform(5, 30)
             if kb > 0:
                 t = max(t, prev_retire)                  # wgmma.wait_group(1): block g - 1 retired
-                release_block(g - 1, t)
+                ring.release(g - 1, w, t)
             prev_retire = retire
         loops.append((start, t, w))
         if i + 1 < n_tiles:
             handed[1 - w] = t + rng.uniform(0.1, 1)
         t = max(t, prev_retire)                          # wgmma.wait_group(0)
-        release_block(i * nk + nk - 1, t)
+        ring.release(i * nk + nk - 1, w, t)
         t = max(t, res_land) + rng.uniform(5, 40)        # cp.async.wait_group(0), epilogue into the staging tile
         if early_refill:
             next_fetch[w] = t
         t += rng.uniform(5, 40)                          # copy-out
         copy_done[w] = t
         t_wg[w] = t
-    produce_until(n_tiles * nk)
     loops.sort()
     assert [w for _, _, w in loops] == [i % 2 for i in range(n_tiles)], "the K loops do not take turns 0, 1, 0, 1, ..."
     for (s0, e0, _), (s1, _, _) in zip(loops, loops[1:]):
@@ -555,9 +576,9 @@ def simulate_linear_ws(rng: random.Random, n_tiles: int, nk: int, stages: int, a
 
 # ---------------------------------------------------------------------------------------------------------- conv A tiles by TMA
 def conv_ws_rules():
-    """checks that gemm_linear_ws.cu / gemm_wgmma.cu still dispatch the conv modes, place each box and walk the taps as
+    """checks that gemm_ws.cu / gemm_wgmma.cu still dispatch the conv modes, place each box and walk the taps as
     conv_ws_box, conv_box_origin and tma_a_tile restate them"""
-    s = _src("gemm_linear_ws.cu")
+    s = _src("gemm_ws.cu")
     for rule in ("if (p.stride != 1 || BM % p.Wo != 0) return false;", "if (hw % BM != 0) return false;",
                  "box[0] = p.Wo, box[1] = BM / p.Wo, box[2] = 1;", "if (BM % hw != 0) return false;",
                  "box[0] = p.Wo, box[1] = p.Ho, box[2] = BM / hw;", "if (p.HW % BM == 0) box[0] = BM, box[1] = 1, box[2] = 1;",
@@ -566,9 +587,9 @@ def conv_ws_rules():
                  "P.y_off = g.up2 ? g.py - 1 : -1;", "P.ax = g.HW, P.ay = g.F, P.taps_w = 1;", "P.x_off = 0;", "P.y_off = -1;",
                  "const unsigned b4[4] = {64, box[0], box[1], box[2]};",
                  "bx = m0 % P.ax + P.x_off;", "by = m0 / P.ax % P.ay + P.y_off;", "bn = m0 / (P.ax * P.ay);",
-                 "tma_load_4d(sA(s), &P.ta, &full[s], c0, bx + kx, by, bn);", "if ((c0 += BK) == p.Cin) {",
+                 "tma_load_4d(sA(s), &P.ta, bar, c0, bx + kx, by, bn);", "if ((c0 += BK) == p.Cin) {",
                  "if (++kx == P.taps_w) kx = 0, ++by;"):
-        assert rule in s, f"gemm_linear_ws.cu no longer contains {rule!r}: update the model"
+        assert rule in s, f"gemm_ws.cu no longer contains {rule!r}: update the model"
     assert "if (conv_ws_box(p, box)) return gemm_conv_ws(p, box, static_cast<int>(tiles), stream);" in _src("gemm_wgmma.cu")
     return True
 
@@ -589,7 +610,7 @@ def conv_geometry(mode: str, **g):
 
 
 def conv_ws_box(p):
-    """gemm_linear_ws.cu conv_ws_box: (bx, by, bn), or None when the conv stays on gemm_wgmma_kernel"""
+    """gemm_ws.cu conv_ws_box: (bx, by, bn), or None when the conv stays on gemm_wgmma_kernel"""
     if p["mode"] == "conv":
         hw = p["Ho"] * p["Wo"]
         if p["stride"] != 1 or 128 % p["Wo"]:
@@ -705,17 +726,17 @@ def check_conv_tma_tiles(mode: str, box=None, **kw):
 # ---------------------------------------------------------------------------------------------------------- persistent fused temporal attention
 def tattn_ws_constants():
     """(stages at n_v = 1, stages at n_v = 3, empty-barrier arrivals) of tattn_fused_kernel's projection ring, as written in
-    attention_wgmma.cu; also checks the item order, block counter and parities the models below restate"""
+    attention_wgmma.cu; also checks the item order and block numbering the models below restate"""
     s = _src("attention_wgmma.cu")
+    k = kernel_body("attention_wgmma.cu", "tattn_fused_kernel")
     m = re.search(r"tattn_stages\(\) \{ return NV == 1 \? (\d+) : (\d+); \}", s)
-    k = s[s.index("tattn_fused_kernel(const"):]
-    arrivals = int(re.search(r"mbar_init\(&empty\[s\], (\d+)\);", k).group(1))
+    arrivals = int(re.search(r"ring\.init\((\d+)\);", k).group(1))
     for rule in ("for (int item = blockIdx.x; item < p.items; item += gridDim.x)", "h = item % p.heads;",
-                 "pix0 = item % p.pix_tiles * p.ppt;", "clip = item / p.pix_tiles;",
-                 "if (g >= S) mbar_wait<false>(&empty[s], ((g / S) - 1) & 1);", "mbar_wait<false>(&full[s], ((g + kb) / S) & 1);",
-                 "mbar_arrive(&empty[(g + kb - 1) % S]);", "mbar_arrive(&empty[(g + nk - 1) % S]);",
-                 "tma_load_4d(sX(s), &p.tx, &full[s], kb * 64, 0, pix0, clip + b * p.src_clips);",
-                 "const unsigned box[4] = {64, static_cast<unsigned>(a->F), static_cast<unsigned>(p.ppt), 1};",
+                 "pix0 = item % p.pix_tiles * p.ppt;", "clip = item / p.pix_tiles;", "for (int kb = 0; kb < nk; ++kb, ++g) {",
+                 "ring.wait(g + kb);", "if (kb > 0) ring.release(g + kb - 1);", "ring.release(g + nk - 1);", "g += nk;",
+                 "tma_load_4d(sX(s), &p.tx, bar, kb * 64, 0, pix0, clip + b * p.src_clips);"):
+        assert rule in k, f"tattn_fused_kernel no longer contains {rule!r}: update the model"
+    for rule in ("const unsigned box[4] = {64, static_cast<unsigned>(a->F), static_cast<unsigned>(p.ppt), 1};",
                  "const unsigned long long strides[3] = {frame, row, frame * a->F};",
                  "items < sm_count_cached() ? items : sm_count_cached()"):
         assert rule in s, f"attention_wgmma.cu no longer contains {rule!r}: update the model"
@@ -742,58 +763,28 @@ def tattn_ws_schedule(clips: int, pix_tiles: int, heads: int, sms: int):
     return True
 
 
-def simulate_tattn_ring(rng: random.Random, n_items: int, passes: int, nk: int, stages: int, arrivals: int = 8,
-                        release: bool = True, wrong_parity: str = "", overrun: bool = False):
-    """tattn_fused_kernel's projection ring over the CTA's items.  Producer: per global block g (item, pass, kb in order), wait
-    empty[g % S] with parity ((g / S) - 1) & 1 (g >= S; skipped when overrun), then TMA into stage g % S.  Consumers w = 0, 1
-    (4 warps each): per block wait full[g % S] with parity (g / S) & 1, issue, wait_group(1) -> each warp releases block g - 1;
-    after a pass's last block wait_group(0) and release it; between items an attention phase of random length.  Asserts: no
-    block is read before it landed, no stage is refilled before both consumers released it.  Negative controls:
-    release=False (consumer 1 never releases), wrong_parity="consumer" / "producer", overrun=True."""
-    n = n_items * passes * nk
-    full = [_MBar(1) for _ in range(stages)]
-    empty = [_MBar(arrivals) for _ in range(stages)]
-    land, released = {}, {}
-    t_prod, g_prod = 0.0, 0
+def simulate_tattn_ring(rng: random.Random, n_items: int, passes: int, nk: int, stages: int, arrivals: int = 8, **faults):
+    """tattn_fused_kernel's projection over the CTA's items on the ring (RingModel, block g = the CTA's g-th K block, item,
+    pass and kb in order).  Consumers w = 0, 1: per block wait for it, issue, wait_group(1) -> release block g - 1; after a
+    pass's last block wait_group(0) and release it; after an item's last pass an attention phase of random length.
+    Negative controls: RingModel's faults."""
+    ring = RingModel(rng, stages, arrivals, 2, **faults)
     t_wg = [rng.uniform(0, 5), rng.uniform(0, 5)]
-
-    def produce_until(limit):
-        nonlocal t_prod, g_prod
-        while g_prod < min(limit, n):
-            g = g_prod
-            s = g % stages
-            if g >= stages:
-                if not overrun:
-                    if len(empty[s].done) < (g // stages) and wrong_parity != "producer":
-                        return  # the stage's release has not happened yet in this replay
-                    t_prod = empty[s].wait((((g // stages) - 1) & 1) ^ (wrong_parity == "producer"), t_prod)
-                for w in range(2):
-                    assert released.get((g - stages, w), float("inf")) <= t_prod, \
-                        f"stage {s} refilled with block {g} while block {g - stages} is read"
-            t_prod += rng.uniform(0.1, 2)
-            land[g] = t_prod + rng.uniform(5, 60)
-            full[s].arrive(land[g])
-            g_prod += 1
-
     retire = {}
-    for g in range(n):
-        produce_until(g + stages)
-        assert g < g_prod, f"block {g} is never loaded (deadlock)"
+    for g in range(n_items * passes * nk):
         kb = g % nk
         for w in range(2):
-            t = full[g % stages].wait(((g // stages) & 1) ^ (wrong_parity == "consumer"), t_wg[w])
-            assert land[g] <= t, f"warpgroup {w} reads block {g} before it landed"
+            t = ring.wait(g, w, t_wg[w])
             retire[(g, w)] = t + rng.uniform(5, 40)
-            t = max(t, retire.get((g - 1, w), 0.0)) if kb > 0 else t  # wait_group(1): block g - 1 retired
-            for b in ([g - 1] if kb > 0 else []) + ([g] if kb == nk - 1 else []):
-                if release or w == 0:
-                    done = max(t, retire[(b, w)])
-                    released[(b, w)] = done
-                    empty[b % stages].arrive(done, arrivals // 2)
-            t_wg[w] = max(t, retire[(g, w)]) if kb == nk - 1 else t
-            if kb == nk - 1 and (g // nk) % passes == passes - 1:
-                t_wg[w] += rng.uniform(10, 80)  # the item's attention and stores
-        produce_until(g + 1 + stages)
+            if kb > 0:
+                t = max(t, retire[(g - 1, w)])  # wait_group(1): block g - 1 retired
+                ring.release(g - 1, w, t)
+            if kb == nk - 1:
+                t = max(t, retire[(g, w)])      # wait_group(0)
+                ring.release(g, w, t)
+                if (g // nk) % passes == passes - 1:
+                    t += rng.uniform(10, 80)    # the item's attention and stores
+            t_wg[w] = t
     return True
 
 
