@@ -55,14 +55,21 @@ __device__ __forceinline__ float gelu_erf_fast(float g) {
 
 // ---- staged epilogue.  A 128 x 128 output tile is packed in fp16 into a staging tile in shared memory (128 rows x 256
 // bytes, 16-byte chunk c of row r at chunk c ^ (r & 7): the 8 rows x 4 lanes of a fragment store and the 8 chunks a quarter
-// warp copies out both cover the 32 banks once) and leaves it in 16-byte stores along the output rows.  A warp's unit of
-// work is a band: the 16 tile rows r0 .. r0 + 15 it holds in one m64n128 accumulator (float[64]); a warp with kBands
-// accumulators owns the bands r0 + 64 b.  A warp fetches, writes and copies out only its own bands' rows, so the kernels
-// order these steps with __syncwarp.  N, ldo and slot_stride are multiples of 8, so every chunk is whole: it is stored iff
-// its row < M and its first column < N.  A value is rounded once: acc + bias + rowbias + residual in fp32, packed over the
-// residual's place in the tile.
+// warp copies out both cover the 32 banks once) and leaves it in 16-byte stores along the output rows.  A 128 x 160 tile
+// (gemm_ws_kernel's 160-column tiles) keeps that layout for its first 128 columns and puts its last 32 (chunks 16 .. 19) in
+// a second part of 128 rows x 64 bytes behind the first, chunk 16 + c of row r at chunk c ^ ((r >> 1) & 3): 8 consecutive
+// rows of a fragment store again cover the 32 banks once, and the tail's copy-out and residual fetch, 8 rows x 4 chunks
+// per warp instruction, read and write 2 whole rows = 128 bytes per quarter warp.  A warp's unit of work is a band: the 16
+// tile rows r0 .. r0 + 15 it holds in one m64nBN accumulator (float[BN / 2]); a warp with kBands accumulators owns the bands
+// r0 + 64 b.  A warp fetches, writes and copies out only its own bands' rows, so the kernels order these steps with
+// __syncwarp.  N, ldo and slot_stride are multiples of 8, so every chunk is whole: it is stored iff its row < M and its
+// first column < N.  A value is rounded once: acc + bias + rowbias + residual in fp32, packed over the residual's place in
+// the tile.
+template <int kBN = 128>
 __device__ __forceinline__ uint32_t stage_offset(int row, int chunk) {
-  return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));
+  static_assert(kBN == 128 || kBN == 160, "staging tiles are 128 or 160 columns wide");
+  if (kBN == 128 || chunk < 16) return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));
+  return static_cast<uint32_t>(128 * 256 + row * 64 + (((chunk - 16) ^ ((row >> 1) & 3)) << 4));
 }
 
 // The row mapping and the output tile differ by A mode, fixed at compile time so that neither instantiation carries the
@@ -79,8 +86,8 @@ __device__ __forceinline__ long long out_row_offset(const GemmP& p, int m) {
 }
 
 // the band at tile rows r0 .. r0 + 15 of the residual tile of `slot` -> staging tile by cp.async: per instruction 2 rows x
-// 16 chunks, zero-filled past M / N
-template <bool kConv>
+// 16 chunks (a 160-wide tile's last 32 columns: 8 rows x 4 chunks), zero-filled past M / N
+template <bool kConv, int kBN = 128>
 __device__ __forceinline__ void fetch_residual_band(const GemmP& p, int slot, int m0, int n0, int r0, uint32_t tile) {
   const int lane = threadIdx.x & 31, ch = lane & 15;
   const int c = n0 + 8 * ch;
@@ -89,15 +96,26 @@ __device__ __forceinline__ void fetch_residual_band(const GemmP& p, int slot, in
   for (int i = 0; i < 8; ++i) {
     const int r = r0 + 2 * i + (lane >> 4);
     const bool v = m0 + r < p.M && c < p.N;
-    cp_async16(tile + stage_offset(r, ch), v ? src + out_row_offset<kConv>(p, m0 + r) : p.residual, v);
+    cp_async16(tile + stage_offset<kBN>(r, ch), v ? src + out_row_offset<kConv>(p, m0 + r) : p.residual, v);
+  }
+  if constexpr (kBN == 160) {
+    const int ct = 16 + (lane & 3), c1 = n0 + 8 * ct;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int r = r0 + 8 * i + (lane >> 2);
+      const bool v = m0 + r < p.M && c1 < p.N;
+      cp_async16(tile + stage_offset<kBN>(r, ct),
+                 v ? p.residual + slot * p.slot_stride + c1 + out_row_offset<kConv>(p, m0 + r) : p.residual, v);
+    }
   }
 }
 
 // acc + bias + rowbias (+ the residual the tile holds) of the warp's bands -> fp16 pairs in fragment order in the staging
 // tile.  Column pair j is the outer loop, so its bias is loaded once for every band (st.shared clobbers memory).
-template <int kBands>
-__device__ __forceinline__ void epilogue_bands(const GemmP& p, const float (&d)[kBands][64], int m0, int n0, int r0,
+template <int kBands, int kAcc>
+__device__ __forceinline__ void epilogue_bands(const GemmP& p, const float (&d)[kBands][kAcc], int m0, int n0, int r0,
                                                uint32_t tile) {
+  constexpr int kBN = 2 * kAcc;  // m64nBN: BN / 2 accumulators per thread
   const int fr = r0 + ((threadIdx.x & 31) >> 2);  // the thread's rows fr + 64 b + 8 h (accumulator layout, acc_row)
   const int cq = 2 * (threadIdx.x & 3);
   const __half* rb[kBands][2];
@@ -109,7 +127,7 @@ __device__ __forceinline__ void epilogue_bands(const GemmP& p, const float (&d)[
       rb[b][h] = p.rowbias && m < p.M ? p.rowbias + static_cast<long long>(m / p.rows_per_rowbias) * p.N : nullptr;
     }
 #pragma unroll
-  for (int j = 0; j < 16; ++j) {
+  for (int j = 0; j < kBN / 8; ++j) {
     const int c = n0 + 8 * j + cq;
     if (c >= p.N) continue;
     float2 bias = make_float2(0.f, 0.f);
@@ -118,7 +136,7 @@ __device__ __forceinline__ void epilogue_bands(const GemmP& p, const float (&d)[
     for (int b = 0; b < kBands; ++b)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const uint32_t at = tile + stage_offset(fr + 64 * b + 8 * h, j) + 2 * cq;
+        const uint32_t at = tile + stage_offset<kBN>(fr + 64 * b + 8 * h, j) + 2 * cq;
         float o0 = d[b][4 * j + 2 * h], o1 = d[b][4 * j + 2 * h + 1];
         if (p.bias) {
           o0 += bias.x;
@@ -141,11 +159,11 @@ __device__ __forceinline__ void epilogue_bands(const GemmP& p, const float (&d)[
 }
 
 // the band at tile rows r0 .. r0 + 15 of the staging tile -> slot `slot` of out: lane -> 16-byte chunk of a row, a warp
-// instruction covers 2 rows x 256 bytes (GEGLU: 4 rows x 128 bytes)
-template <bool kConv>
+// instruction covers 2 rows x 256 bytes (GEGLU: 4 rows x 128 bytes; a 160-wide tile's last 32 columns: 8 rows x 64 bytes)
+template <bool kConv, int kBN = 128>
 __device__ __forceinline__ void copy_out_band(const GemmP& p, int slot, int m0, int n0, int r0, uint32_t tile) {
   const int lane = threadIdx.x & 31;
-  const bool geglu = !kConv && p.geglu;
+  const bool geglu = kBN == 128 && !kConv && p.geglu;  // GEGLU tiles are 128 wide
   const int lg = geglu ? 3 : 4;  // log2(chunks per output row of the tile)
   const int col0 = geglu ? n0 / 2 : n0, n_out = geglu ? p.N / 2 : p.N;
   __half* out = p.out + slot * p.slot_stride + col0;
@@ -154,12 +172,23 @@ __device__ __forceinline__ void copy_out_band(const GemmP& p, int slot, int m0, 
     const int idx = 32 * i + lane;
     const int r = r0 + (idx >> lg), ch = idx & ((1 << lg) - 1);
     if ((idx >> lg) < 16 && m0 + r < p.M && col0 + 8 * ch < n_out)
-      st_global_v4(out + out_row_offset<kConv>(p, m0 + r) + 8 * ch, ld_shared_v4(tile + stage_offset(r, ch)));
+      st_global_v4(out + out_row_offset<kConv>(p, m0 + r) + 8 * ch, ld_shared_v4(tile + stage_offset<kBN>(r, ch)));
+  }
+  if constexpr (kBN == 160) {
+    const int ct = 16 + (lane & 3);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int r = r0 + 8 * i + (lane >> 2);
+      if (m0 + r < p.M && n0 + 8 * ct < p.N)
+        st_global_v4(out + out_row_offset<kConv>(p, m0 + r) + 8 * ct, ld_shared_v4(tile + stage_offset<kBN>(r, ct)));
+    }
   }
 }
 
 // Launches of gemm_ws.cu's persistent kernel on `tiles` output tiles; p is validated and filled by av2v_gemm_f16.
-// LINEAR mode; a conv mode whose tiles are each one box of its input (conv_ws_box returns true and the box).
+// LINEAR mode; a conv mode whose tiles are each one box of its input (conv_ws_box returns true and the box).  ws_tile_n is
+// the column tile of both (128 or 160): av2v_gemm_f16 counts p.n_tiles in it.
+int ws_tile_n(const GemmP& p);
 int gemm_linear_ws(const GemmP& p, int tiles, cudaStream_t stream);
 bool conv_ws_box(const GemmP& p, unsigned (&box)[3]);
 int gemm_conv_ws(const GemmP& p, const unsigned (&box)[3], int tiles, cudaStream_t stream);

@@ -267,12 +267,14 @@ extern "C" int av2v_gemm_f16(const av2v_gemm_args* a, av2v_stream_t stream_) {
     return fail(AV2V_EINVAL, "gemm: unknown A mode %d", a->mode);
   }
   p.num_kb = (a->K + BK - 1) / BK;
-  p.n_tiles = (a->N + BN - 1) / BN;
+  unsigned box[3];
+  const bool ws = p.mode == AV2V_A_LINEAR || conv_ws_box(p, box);
+  const int bn = ws ? ws_tile_n(p) : BN;
+  p.n_tiles = (a->N + bn - 1) / bn;
   const long long tiles = static_cast<long long>((a->M + BM - 1) / BM) * p.n_tiles;
   AV2V_REQUIRE(tiles < (1ll << 31), AV2V_ENOSUP, "gemm: too many tiles");
   if (p.mode == AV2V_A_LINEAR) return gemm_linear_ws(p, static_cast<int>(tiles), stream);
-  unsigned box[3];
-  if (conv_ws_box(p, box)) return gemm_conv_ws(p, box, static_cast<int>(tiles), stream);
+  if (ws) return gemm_conv_ws(p, box, static_cast<int>(tiles), stream);
   static bool attr_set = false;
   if (!attr_set) {
     AV2V_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));

@@ -8,12 +8,12 @@
 // (tile blockIdx.x + i * gridDim.x, column tiles fastest, so the CTAs running at one time share A row blocks in L2) with
 // three warpgroups:
 //   producer (warpgroup 0, registers lowered): one thread issues the TMA loads of every K block g = i * num_kb + kb of the
-//     CTA into a kStages ring (ring.cuh) of 32 KB stages (A 128 x 64 and W 128 x 64 boxes, 128-byte swizzle = the sw128
-//     layout the wgmma descriptors read; TMA zero-fills ragged M / N, the K tail and the columns past k_split of a
+//     CTA into a kStages ring (ring.cuh) of 32 / 36 KB stages (A 128 x 64 and W BN x 64 boxes, 128-byte swizzle = the
+//     sw128 layout the wgmma descriptors read; TMA zero-fills ragged M / N, the K tail and the columns past k_split of a
 //     two-source A).  It runs ahead across tile boundaries, so the next tile's first blocks land under this tile's last MMAs
 //     and epilogue (tools/kernel_models.py models this schedule).
 //   consumers (warpgroups 1, 2, registers raised): warpgroup w takes the CTA's tiles i = w, w + 2, ... whole: 128 rows x
-//     128 columns as two wgmma.m64n128k16 per k16 step (rows 0-63, 64-127) into 128 fp32 accumulators per thread.  Their
+//     BN columns as two wgmma.m64nBNk16 per k16 step (rows 0-63, 64-127) into BN fp32 accumulators per thread.  Their
 //     K loops take turns (math order 0, 1, 0, 1, ...): a warpgroup hands the tensor cores over once it has issued its last
 //     MMA of a tile and runs its epilogue under the other's K loop.
 //
@@ -29,11 +29,15 @@
 //     box with 128-byte rows is the same sw128 tile whatever its shape, and every block holds the values gemm_wgmma.cu's
 //     cp.async gather puts there, so K order, sum order and results are those of gemm_wgmma_kernel.
 //
-// Epilogue: gemm_common.cuh's staged epilogue, shared with gemm_wgmma_kernel; GEGLU pairs the h and gate columns that
-// geglu_pack interleaves, output tile 128 x 64.  Each consumer warpgroup has its own 32 KB staging tile; each warp owns two
-// bands (rows 16 w .. 16 w + 15 and 64 + 16 w .., one per accumulator) and fetches their residual chunks by cp.async
-// before its K loop, so a warp needs only __syncwarp: all of a warp's residual reads complete before its first store (a
-// residual that aliases out stays safe), and its copy-out reads complete before the next tile's residual fetch or stores
+// The column tile BN is 128, or 160 where N is a multiple of 160 and the wider tiles shorten the schedule (ws_tile_n): the
+// 64 x 64 level's N = 320 and 960 then run as whole tiles, and each A block feeds 160 columns.  At 160 the ring
+// (4 x 36 KB) and the two staging tiles (2 x 40 KB) take 225 KB of shared memory.
+//
+// Epilogue: gemm_common.cuh's staged epilogue, shared with gemm_wgmma_kernel; GEGLU (BN = 128 only) pairs the h and gate
+// columns that geglu_pack interleaves, output tile 128 x 64.  Each consumer warpgroup has its own 32 / 40 KB staging
+// tile; each warp owns two bands (rows 16 w .. 16 w + 15 and 64 + 16 w .., one per accumulator) and fetches their
+// residual chunks by cp.async before its K loop, so a warp needs only __syncwarp: all of a warp's residual reads complete
+// before its first store (a residual that aliases out stays safe), and its copy-out reads complete before the next tile's residual fetch or stores
 // refill the tile.  Conv with a residual in several slots (PnP conv injection) runs the slots one after another through
 // the one staging tile: fetch residual s (slot 0's before the K loop), epilogue, copy out to slot s, __syncwarp; without a
 // residual the one tile is copied to every slot.  An up2 phase writes its rows to the phase's pixels of the 2x output.
@@ -43,13 +47,14 @@
 namespace av2v {
 namespace {
 
-constexpr int BM = 128, BN = 128, BK = 64;
+constexpr int BM = 128, BK = 64;
 constexpr int kStages = 4;
 constexpr int kThreads = 384;
-constexpr int kTileBytes = BM * BK * 2;                // 16 KB: A and W boxes alike (BM == BN)
-constexpr int kStageBytes = 2 * kTileBytes;
-constexpr int kStagingBytes = BM * BN * 2;             // 32 KB per consumer warpgroup
-constexpr int kSmemBytes = kStages * kStageBytes + 2 * kStagingBytes + 1024;
+constexpr int kTileBytes = BM * BK * 2;                       // 16 KB: the A box
+template <int kBN> constexpr int kStageBytes = kTileBytes + kBN * BK * 2;  // + the W box: 32 / 36 KB
+template <int kBN> constexpr int kStagingBytes = BM * kBN * 2;             // 32 / 40 KB per consumer warpgroup
+template <int kBN> constexpr int kSmemBytes = kStages * kStageBytes<kBN> + 2 * kStagingBytes<kBN> + 1024;
+static_assert(kSmemBytes<160> <= 227 * 1024, "the 160-wide ring and staging tiles must fit an SM's shared memory");
 
 struct WsP {
   CUtensorMap ta, ta2, tw;  // A (LINEAR: columns [0, k_split); conv: the input tensor), second source (columns [k_split, K)), W [N][K]
@@ -90,14 +95,15 @@ __device__ __forceinline__ void geglu_epilogue(const GemmP& p, float (&d)[2][64]
   }
 }
 
-template <bool kConv>
+template <bool kConv, int kBN>
 __global__ void __launch_bounds__(kThreads, 1) gemm_ws_kernel(const __grid_constant__ WsP P) {
+  constexpr int kStage = kStageBytes<kBN>, kStaging = kStagingBytes<kBN>;
   const GemmP& p = P.g;
   extern __shared__ uint8_t smem_raw[];
   __shared__ StageRing<kStages> ring;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t s0 = smem_u32(smem);
-  auto sA = [&](int s) { return s0 + static_cast<uint32_t>(s) * kStageBytes; };
+  auto sA = [&](int s) { return s0 + static_cast<uint32_t>(s) * kStage; };
   auto sB = [&](int s) { return sA(s) + kTileBytes; };
   const int nk = p.num_kb;
   if (threadIdx.x == 0) {
@@ -112,7 +118,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_ws_kernel(const __grid_const
     if (threadIdx.x == 0) {
       int g = 0;
       for (int t = blockIdx.x; t < P.tiles; t += gridDim.x) {
-        const int m0 = t / p.n_tiles * BM, n0 = t % p.n_tiles * BN;
+        const int m0 = t / p.n_tiles * BM, n0 = t % p.n_tiles * kBN;
         int bx = 0, by = 0, bn = 0, c0 = 0, kx = 0;  // conv: the tile's box origin, block kb's channel and tap column
         if constexpr (kConv) {
           bx = m0 % P.ax + P.x_off;
@@ -121,7 +127,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_ws_kernel(const __grid_const
         }
         for (int kb = 0; kb < nk; ++kb, ++g) {
           const int s = ring.stage(g), k0 = kb * BK;
-          uint64_t* bar = ring.produce(g, kStageBytes);
+          uint64_t* bar = ring.produce(g, kStage);
           if constexpr (kConv) {  // block kb = tap (ky, kx), channels c0 .. c0 + 63; walked without divisions
             tma_load_4d(sA(s), &P.ta, bar, c0, bx + kx, by, bn);
             if ((c0 += BK) == p.Cin) {
@@ -140,24 +146,24 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_ws_kernel(const __grid_const
   // ---- consumers
   setmaxnreg_inc<232>();
   const int wg = role - 1;
-  const uint32_t staging = s0 + kStages * kStageBytes + wg * kStagingBytes;
+  const uint32_t staging = s0 + kStages * kStage + wg * kStaging;
   turn_open(wg);  // a warpgroup hands over only when another tile follows: every sync has exactly one matching arrive
 
   const int r0 = 16 * ((threadIdx.x >> 5) & 3);  // the warp's bands: tile rows r0 .. r0 + 15 and r0 + 64 ..
-  float d[2][64];
+  float d[2][kBN / 2];
   for (int i = wg, t = blockIdx.x + wg * gridDim.x; t < P.tiles; i += 2, t += 2 * gridDim.x) {
-    const int m0 = t / p.n_tiles * BM, n0 = t % p.n_tiles * BN;
+    const int m0 = t / p.n_tiles * BM, n0 = t % p.n_tiles * kBN;
     if (p.residual)
 #pragma unroll
       for (int b = 0; b < 2; ++b) {
-        if constexpr (kConv) fetch_residual_band<true>(p, 0, m0, n0, r0 + 64 * b, staging);
-        else fetch_residual_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);
+        if constexpr (kConv) fetch_residual_band<true, kBN>(p, 0, m0, n0, r0 + 64 * b, staging);
+        else fetch_residual_band<false, kBN>(p, 0, m0, n0, r0 + 64 * b, staging);
       }
     cp_async_commit();
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
-      for (int e = 0; e < 64; ++e) d[h][e] = 0.f;
+      for (int e = 0; e < kBN / 2; ++e) d[h][e] = 0.f;
     const int g0 = i * nk;
     turn_take(wg);
     for (int kb = 0; kb < nk; ++kb) {
@@ -167,8 +173,13 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_ws_kernel(const __grid_const
 #pragma unroll
       for (int k = 0; k < BK / 16; ++k) {
         const uint64_t db = sw128_desc(sB(s) + k * 32);
-        wgmma_m64n128_ss(d[0], sw128_desc(sA(s) + k * 32), db, 1);
-        wgmma_m64n128_ss(d[1], sw128_desc(sA(s) + 64 * 128 + k * 32), db, 1);
+        if constexpr (kBN == 128) {
+          wgmma_m64n128_ss(d[0], sw128_desc(sA(s) + k * 32), db, 1);
+          wgmma_m64n128_ss(d[1], sw128_desc(sA(s) + 64 * 128 + k * 32), db, 1);
+        } else {
+          wgmma_m64n160_ss(d[0], sw128_desc(sA(s) + k * 32), db, 1);
+          wgmma_m64n160_ss(d[1], sw128_desc(sA(s) + 64 * 128 + k * 32), db, 1);
+        }
       }
       wgmma_commit();
       wgmma_wait<1>();
@@ -189,7 +200,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_ws_kernel(const __grid_const
       for (int sl = 0; sl < n_res; ++sl) {
         if (sl > 0) {  // the copy-out of slot sl - 1 has read the warp's rows (__syncwarp below)
 #pragma unroll
-          for (int b = 0; b < 2; ++b) fetch_residual_band<true>(p, sl, m0, n0, r0 + 64 * b, staging);
+          for (int b = 0; b < 2; ++b) fetch_residual_band<true, kBN>(p, sl, m0, n0, r0 + 64 * b, staging);
           cp_async_commit();
         }
         cp_async_wait<0>();
@@ -199,37 +210,56 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_ws_kernel(const __grid_const
 #pragma unroll 1
         for (int o = p.residual ? sl : 0; o < (p.residual ? sl + 1 : p.n_slots); ++o)
 #pragma unroll 1
-          for (int b = 0; b < 2; ++b) copy_out_band<true>(p, o, m0, n0, r0 + 64 * b, staging);
+          for (int b = 0; b < 2; ++b) copy_out_band<true, kBN>(p, o, m0, n0, r0 + 64 * b, staging);
         __syncwarp();  // every lane's copy-out reads are done before the next slot or tile refills the warp's rows
       }
     } else {
       cp_async_wait<0>();
       __syncwarp();  // the residual chunks this warp's lanes fetched for each other have landed
-      if (p.geglu) geglu_epilogue(p, d, n0, staging);
-      else epilogue_bands<2>(p, d, m0, n0, r0, staging);
+      if constexpr (kBN == 128) {
+        if (p.geglu) geglu_epilogue(p, d, n0, staging);
+        else epilogue_bands<2>(p, d, m0, n0, r0, staging);
+      } else {
+        epilogue_bands<2>(p, d, m0, n0, r0, staging);  // GEGLU runs on 128-wide tiles (ws_tile_n)
+      }
       __syncwarp();
 #pragma unroll
-      for (int b = 0; b < 2; ++b) copy_out_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);
+      for (int b = 0; b < 2; ++b) copy_out_band<false, kBN>(p, 0, m0, n0, r0 + 64 * b, staging);
       __syncwarp();  // every lane's copy-out reads are done before the next tile refills the warp's rows
     }
   }
 }
 
-template <bool kConv>
-int launch_ws(const WsP& P, cudaStream_t stream) {
+template <bool kConv, int kBN>
+int launch_ws(WsP P, cudaStream_t stream) {
+  const GemmP& g = P.g;
+  if (int e = encode_rows_map(&P.tw, g.w, g.K, g.N, 1, 1, g.K, 0, kBN)) return e;
   static bool attr_set = false;  // one per instantiation
   if (!attr_set) {
-    AV2V_CHECK_CUDA(cudaFuncSetAttribute(gemm_ws_kernel<kConv>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+    AV2V_CHECK_CUDA(cudaFuncSetAttribute(gemm_ws_kernel<kConv, kBN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         kSmemBytes<kBN>));
     attr_set = true;
   }
   const int tiles = P.tiles;
   const int grid = static_cast<int>(tiles < sm_count_cached() ? tiles : sm_count_cached());
-  gemm_ws_kernel<kConv><<<grid, kThreads, kSmemBytes, stream>>>(P);
+  gemm_ws_kernel<kConv, kBN><<<grid, kThreads, kSmemBytes<kBN>, stream>>>(P);
   AV2V_CHECK_CUDA(cudaGetLastError());
   return AV2V_OK;
 }
 
 }  // namespace
+
+// The column tile: 160 where it shortens the schedule.  Each CTA runs its tiles one after another, so a GEMM takes about
+// ceil(tiles / SMs) tile times, and a tile's time grows with its width.  160 takes N = 320 and 960 (the 64 x 64 level) as
+// whole tiles instead of 3 and 8 with the last half empty, and at N = 640 or 1280 it feeds each A block to more columns;
+// 128 stays where its extra tiles fill SMs that 160 would leave idle (the 8 x 8 level's 24 row tiles at N = 1280).  GEGLU
+// keeps 128: geglu_pack interleaves its h and gate columns per 128-column tile.
+int ws_tile_n(const GemmP& p) {
+  if (p.geglu || p.N % 160 != 0) return 128;
+  const long long mt = (p.M + BM - 1) / BM, sms = sm_count_cached();
+  const long long t128 = (mt * ((p.N + 127) / 128) + sms - 1) / sms * 128, t160 = (mt * (p.N / 160) + sms - 1) / sms * 160;
+  return t160 <= t128 ? 160 : 128;
+}
 
 int gemm_linear_ws(const GemmP& g, int tiles, cudaStream_t stream) {
   WsP P{};
@@ -238,9 +268,8 @@ int gemm_linear_ws(const GemmP& g, int tiles, cudaStream_t stream) {
   P.ta2 = P.ta;
   if (g.a2 != nullptr)
     if (int e = encode_rows_map(&P.ta2, g.a2, g.K - g.k_split, g.M, 1, 1, g.lda2, 0, BM)) return e;
-  if (int e = encode_rows_map(&P.tw, g.w, g.K, g.N, 1, 1, g.K, 0, BN)) return e;
   P.tiles = tiles;
-  return launch_ws<false>(P, stream);
+  return ws_tile_n(g) == 160 ? launch_ws<false, 160>(P, stream) : launch_ws<false, 128>(P, stream);
 }
 
 // A conv runs here iff the 128 output rows of every tile are one box of its input, in row order:
@@ -298,9 +327,8 @@ int gemm_conv_ws(const GemmP& g, const unsigned (&box)[3], int tiles, cudaStream
     P.y_off = -1;
   }
   P.ta2 = P.ta;
-  if (int e = encode_rows_map(&P.tw, g.w, g.K, g.N, 1, 1, g.K, 0, BN)) return e;
   P.tiles = tiles;
-  return launch_ws<true>(P, stream);
+  return ws_tile_n(g) == 160 ? launch_ws<true, 160>(P, stream) : launch_ws<true, 128>(P, stream);
 }
 
 }  // namespace av2v

@@ -183,6 +183,21 @@ __device__ __forceinline__ void wgmma_m64n128_ss(float (&d)[64], uint64_t da, ui
         AV2V_WG_D8(56)
       : "l"(da), "l"(db), "r"(accumulate));
 }
+// D[64 x 160] (+)= A[64 x 16] * B[16 x 160], both K-major in shared memory (B: a 160-row sw128 box)
+__device__ __forceinline__ void wgmma_m64n160_ss(float (&d)[80], uint64_t da, uint64_t db, int accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %82, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n160k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, "
+      "%80, %81, p, 1, 1, 0, 0;\n}\n"
+      : AV2V_WG_D8(0), AV2V_WG_D8(8), AV2V_WG_D8(16), AV2V_WG_D8(24), AV2V_WG_D8(32), AV2V_WG_D8(40), AV2V_WG_D8(48),
+        AV2V_WG_D8(56), AV2V_WG_D8(64), AV2V_WG_D8(72)
+      : "l"(da), "l"(db), "r"(accumulate));
+}
 #undef AV2V_WG_D8
 
 // Accumulator layout of wgmma m64nN (per warpgroup thread t, warp w = t / 32, lane l): element d[i] is row

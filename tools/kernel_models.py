@@ -225,9 +225,29 @@ def acc_col(t, i):
     return 8 * (i >> 2) + 2 * (t & 3) + (i & 1)
 
 
-def stage_offset(row, chunk, swizzle=True):
-    """gemm_common.cuh stage_offset: byte offset of 16-byte chunk `chunk` of row `row` in the epilogue's staging tile (256-byte rows)"""
-    return row * 256 + ((chunk ^ (row & 7 if swizzle else 0)) << 4)
+def stage_offset(row, chunk, swizzle=True, bn=128, tail_swizzle=True):
+    """gemm_common.cuh stage_offset<bn>: byte offset of 16-byte chunk `chunk` of row `row` in the epilogue's staging tile
+    (256-byte rows; a 160-wide tile's chunks 16 .. 19 in a second part of 64-byte rows behind the first)"""
+    if bn == 128 or chunk < 16:
+        return row * 256 + ((chunk ^ (row & 7 if swizzle else 0)) << 4)
+    return 128 * 256 + row * 64 + (((chunk - 16) ^ ((row >> 1) & 3 if tail_swizzle else 0)) << 4)
+
+
+def copy_out_passes(bn=128, geglu=False):
+    """copy_out_band's (and, for a tile's full width, fetch_residual_band's) passes over a band: (first chunk, log2 chunks
+    per row, warp instructions).  Lane l of instruction i takes chunk first + idx % 2^lg of band row idx >> lg, idx = 32 i + l,
+    if that row is < 16"""
+    if geglu:
+        return [(0, 3, 8)]
+    return [(0, 4, 8)] + ([(16, 2, 2)] if bn == 160 else [])
+
+
+def band_lanes(r0, bn=128, geglu=False):
+    """per warp instruction of copy_out_band: [(lane, row, chunk)]"""
+    for c0, lg, n in copy_out_passes(bn, geglu):
+        for i in range(n):
+            yield [(lane, r0 + ((32 * i + lane) >> lg), c0 + ((32 * i + lane) & ((1 << lg) - 1))) for lane in range(32)
+                   if ((32 * i + lane) >> lg) < 16], c0, lg
 
 
 def epilogue_bands(kernel: str):
@@ -240,53 +260,64 @@ def epilogue_bands(kernel: str):
     return {w: [64 * b + acc_row(32 * w, 0) for b in range(2)] for w in range(4)}
 
 
-def check_epilogue_staging(kernel: str, geglu: bool = False, swizzle: bool = True):
+def check_epilogue_staging(kernel: str, geglu: bool = False, swizzle: bool = True, bn: int = 128, tail_swizzle: bool = True):
     """The staging tile of the GEMM epilogue (gemm_common.cuh), per warp and band (epilogue_bands: a band is the 16 rows a
-    warp holds in one accumulator; conv: 8 warps x 1 band, linear: 4 warps x 2 bands, GEGLU in linear only).  (1)
-    Fragment-order 4-byte writes (and the residual reads at the same addresses): one instruction is 8 rows x 4 lanes; its 32
-    lanes hit 32 different banks, and over all instructions every (row, column pair) of the tile is written exactly once.
-    (2) Copy-out 16-byte reads, lane -> chunk (32 i + lane) of the band's rows in row-major order: each quarter warp (one
-    shared-memory wavefront of a 128-bit access) covers the 8 bank groups once, the lanes of a row read consecutive chunks
-    (whole 128-byte lines of the output row), and every chunk is read exactly once BY THE WARP THAT WROTE IT — the kernels
-    order the two with __syncwarp only.  (3) The residual cp.async pattern (2 rows x 16 chunks per instruction) fetches
-    every chunk once, again in the warp that consumes it.  swizzle=False is the negative control."""
+    warp holds in one accumulator; conv: 8 warps x 1 band, linear: 4 warps x 2 bands, GEGLU in linear only; bn = 160:
+    gemm_ws_kernel's 160-wide tiles, linear only).  (1) Fragment-order 4-byte writes (and the residual reads at the same
+    addresses): one instruction is 8 rows x 4 lanes; its 32 lanes hit 32 different banks, and over all instructions every
+    (row, column pair) of the tile is written exactly once.  (2) Copy-out 16-byte reads (copy_out_passes: lane -> chunk of
+    the band's rows in row-major order, per part of the tile): each quarter warp (one shared-memory wavefront of a 128-bit
+    access) covers the 8 bank groups once, the lanes of a row read consecutive chunks (whole 128-byte lines of the output
+    row, or a 160-wide tile's 64-byte tail), and every chunk is read exactly once BY THE WARP THAT WROTE IT — the kernels
+    order the two with __syncwarp only.  (3) The residual cp.async pattern (2 rows x 16 chunks per instruction; the tail: the
+    copy-out's) fetches every chunk once, again in the warp that consumes it.  swizzle=False / tail_swizzle=False are the
+    negative controls."""
     assert not (geglu and kernel == "conv"), "GEGLU runs on gemm_ws_kernel<false> only"
+    assert bn == 128 or (kernel == "linear" and not geglu), "160-wide tiles are gemm_ws_kernel's, without GEGLU"
     src = _src("gemm_common.cuh")
-    assert "return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));" in src, "stage_offset changed: update the model"
+    assert "if (kBN == 128 || chunk < 16) return static_cast<uint32_t>(row * 256 + ((chunk ^ (row & 7)) << 4));" in src, \
+        "stage_offset changed: update the model"
+    assert "return static_cast<uint32_t>(128 * 256 + row * 64 + (((chunk - 16) ^ ((row >> 1) & 3)) << 4));" in src, \
+        "stage_offset changed: update the model"
+    for rule in ("const int r = r0 + 8 * i + (lane >> 2);", "const int ct = 16 + (lane & 3)", "for (int i = 0; i < 2; ++i) {"):
+        assert src.count(rule) == 2, f"the tail passes of fetch_residual_band / copy_out_band changed ({rule!r}): update the model"
     for f, rule in (("gemm_wgmma.cu", "const int r0 = 16 * (threadIdx.x >> 5);"),
                     ("gemm_ws.cu", "const int r0 = 16 * ((threadIdx.x >> 5) & 3);"),
-                    ("gemm_ws.cu", "fetch_residual_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);"),
-                    ("gemm_ws.cu", "copy_out_band<false>(p, 0, m0, n0, r0 + 64 * b, staging);")):
+                    ("gemm_ws.cu", "fetch_residual_band<false, kBN>(p, 0, m0, n0, r0 + 64 * b, staging);"),
+                    ("gemm_ws.cu", "copy_out_band<false, kBN>(p, 0, m0, n0, r0 + 64 * b, staging);")):
         assert rule in _src(f), f"{f} no longer contains {rule!r}: update the model"
+
+    def so(r, c):
+        return stage_offset(r, c, swizzle, bn, tail_swizzle)
+
     bands = epilogue_bands(kernel)
-    lg = 3 if geglu else 4  # log2(chunks per tile row): the GEGLU output tile is 128 x 64
-    cpr = 1 << lg
+    cpr = 8 if geglu else bn // 8  # chunks per tile row: the GEGLU output tile is 128 x 64
+    tile_bytes = 128 * 2 * bn
     writer = {}  # byte address of a 4-byte word -> warp
     for warp, rows in bands.items():
-        chunks = [4 * g + jj for g in range(2) for jj in range(4)] if geglu else list(range(16))
+        chunks = [4 * g + jj for g in range(2) for jj in range(4)] if geglu else list(range(cpr))
         for r0 in rows:
             for chunk in chunks:
                 for h in range(2):
-                    addrs = [stage_offset(r0 + acc_row(lane, 2 * h), chunk, swizzle) + 4 * (lane & 3) for lane in range(32)]
+                    addrs = [so(r0 + acc_row(lane, 2 * h), chunk) + 4 * (lane & 3) for lane in range(32)]
                     assert len({(a // 4) % 32 for a in addrs}) == 32, f"fragment store of chunk {chunk}: bank conflict"
                     for a in addrs:
-                        assert 0 <= a < 128 * 256 and a not in writer, "staging word written twice"
+                        assert 0 <= a < tile_bytes and a not in writer, "staging word written twice"
                         writer[a] = warp
-    want = {stage_offset(r, c, swizzle) + 4 * q for r in range(128) for c in range(cpr) for q in range(4)}
+    want = {so(r, c) + 4 * q for r in range(128) for c in range(cpr) for q in range(4)}
     assert set(writer) == want, "the fragment stores do not cover the tile"
     read = set()
     for warp, rows in bands.items():
         for r0 in rows:
-            for i in range(8):
-                lanes = [(lane, r0 + ((32 * i + lane) >> lg), (32 * i + lane) & (cpr - 1)) for lane in range(32)
-                         if ((32 * i + lane) >> lg) < 16]
+            for lanes, c0, lg in band_lanes(r0, bn, geglu):
                 for q in range(0, len(lanes), 8):
-                    groups = {(stage_offset(r, c, swizzle) // 16) % 8 for _, r, c in lanes[q:q + 8]}
+                    groups = {(so(r, c) // 16) % 8 for _, r, c in lanes[q:q + 8]}
                     assert len(groups) == 8, "copy-out read: bank conflict inside a quarter warp"
                 for (l0, ra, ca), (l1, rb, cb) in zip(lanes, lanes[1:]):
-                    assert (rb, cb) == ((ra, ca + 1) if ca + 1 < cpr else (ra + 1, 0)), "copy-out lanes are not consecutive chunks"
+                    assert (rb, cb) == ((ra, ca + 1) if ca + 1 < c0 + (1 << lg) else (ra + 1, c0)), \
+                        "copy-out lanes are not consecutive chunks"
                 for _, r, c in lanes:
-                    a = stage_offset(r, c, swizzle)
+                    a = so(r, c)
                     assert a not in read and all(writer[a + 4 * q] == warp for q in range(4)), "chunk read twice or by another warp"
                     read.add(a)
     assert len(read) == 128 * cpr
@@ -294,12 +325,35 @@ def check_epilogue_staging(kernel: str, geglu: bool = False, swizzle: bool = Tru
         fetched = {}
         for warp, rows in bands.items():
             for r0 in rows:
-                for i in range(8):
+                lanes = [(r0 + 2 * i + (lane >> 4), lane & 15) for i in range(8) for lane in range(32)]
+                if bn == 160:
+                    lanes += [(r, c) for ls, c0, _ in band_lanes(r0, bn) if c0 == 16 for _, r, c in ls]
+                for r, c in lanes:
+                    a = so(r, c)
+                    assert a not in fetched and writer[a] == warp, "residual chunk fetched twice or by another warp"
+                    fetched[a] = warp
+        assert len(fetched) == 128 * cpr
+    return True
+
+
+def check_ragged_copy_out(M: int, N: int, m0: int, n0: int, bn: int = 128, passes=None):
+    """The output chunks the copy-out of one tile (m0, n0) stores, over every band of both kernels' band ownership alike
+    (gemm_ws_kernel: 4 warps x 2 bands): every 16-byte chunk of the tile's rows < M and columns < N exactly once, nothing
+    past them.  passes: copy_out_passes(bn) unless given (negative control: drop the tail pass)"""
+    passes = copy_out_passes(bn) if passes is None else passes
+    stored = {}
+    for rows in epilogue_bands("linear").values():
+        for r0 in rows:
+            for c0, lg, n in passes:
+                for i in range(n):
                     for lane in range(32):
-                        a = stage_offset(r0 + 2 * i + (lane >> 4), lane & 15, swizzle)
-                        assert a not in fetched and writer[a] == warp, "residual chunk fetched twice or by another warp"
-                        fetched[a] = warp
-        assert len(fetched) == 128 * 16
+                        idx = 32 * i + lane
+                        r, c = r0 + (idx >> lg), c0 + (idx & ((1 << lg) - 1))
+                        if (idx >> lg) < 16 and m0 + r < M and n0 + 8 * c < N:
+                            stored[(m0 + r, n0 + 8 * c)] = stored.get((m0 + r, n0 + 8 * c), 0) + 1
+    want = {(m, c) for m in range(m0, min(m0 + 128, M)) for c in range(n0, min(n0 + bn, N), 8)}
+    assert set(stored) == want, f"copy-out of tile ({m0}, {n0}) misses or adds chunks"
+    assert all(v == 1 for v in stored.values()), "an output chunk is stored twice"
     return True
 
 
@@ -347,6 +401,7 @@ def check_epilogue(geglu_pack, N_geglu=(128, 256, 2560)):
             assert rows == want
     for kernel, geglu in (("conv", False), ("linear", False), ("linear", True)):
         check_epilogue_staging(kernel, geglu)
+    check_epilogue_staging("linear", bn=160)
     return True
 
 
@@ -488,7 +543,7 @@ def linear_ws_constants():
     stages = int(re.search(r"constexpr int kStages = (\d+);", _src("gemm_ws.cu")).group(1))
     arrivals = int(re.search(r"ring\.init\((\d+)\);", k).group(1))
     for rule in ("StageRing<kStages> ring;", "for (int t = blockIdx.x; t < P.tiles; t += gridDim.x)",
-                 "for (int kb = 0; kb < nk; ++kb, ++g) {", "ring.produce(g, kStageBytes);",
+                 "for (int kb = 0; kb < nk; ++kb, ++g) {", "ring.produce(g, kStage);",
                  "for (int i = wg, t = blockIdx.x + wg * gridDim.x; t < P.tiles; i += 2, t += 2 * gridDim.x)",
                  "const int g0 = i * nk;", "const int g = g0 + kb, s = ring.stage(g);", "ring.wait(g);",
                  "if (kb > 0) ring.release(g - 1);", "ring.release(g0 + nk - 1);", "turn_open(wg);",
@@ -496,6 +551,38 @@ def linear_ws_constants():
         assert rule in k, f"gemm_ws_kernel no longer contains {rule!r}: update the model"
     assert "tiles < sm_count_cached() ? tiles : sm_count_cached()" in _src("gemm_ws.cu")
     return stages, arrivals
+
+
+def ws_tile_n(M: int, N: int, geglu: bool = False, sms: int = 132):
+    """gemm_ws.cu ws_tile_n: the column tile of gemm_ws_kernel (av2v_gemm_f16 counts n_tiles in it): 160 when N is a
+    multiple of 160 and ceil(tiles / SMs) tile widths, the schedule's length, are no longer than at 128"""
+    src = _src("gemm_ws.cu")
+    for r in ("if (p.geglu || p.N % 160 != 0) return 128;",
+              "const long long mt = (p.M + BM - 1) / BM, sms = sm_count_cached();",
+              "const long long t128 = (mt * ((p.N + 127) / 128) + sms - 1) / sms * 128, t160 = (mt * (p.N / 160) + sms - 1) / sms * 160;",
+              "return t160 <= t128 ? 160 : 128;"):
+        assert r in src, f"ws_tile_n no longer contains {r!r}: update the model"
+    for r in ("const int bn = ws ? ws_tile_n(p) : BN;", "p.n_tiles = (a->N + bn - 1) / bn;"):
+        assert r in _src("gemm_wgmma.cu"), f"gemm_wgmma.cu no longer contains {r!r}: update the model"
+    if geglu or N % 160:
+        return 128
+    mt = -(-M // 128)
+    return 160 if -(-mt * N // 160 // sms) * 160 <= -(-mt * -(-N // 128) // sms) * 128 else 128
+
+
+def ws_smem_bytes(bn: int):
+    """gemm_ws_kernel's dynamic shared memory at column tile bn, as gemm_ws.cu sizes it: the ring's stages (A 128 x 64 and
+    W bn x 64 fp16 boxes), one 128 x bn fp16 staging tile per consumer warpgroup and 1 KB to align the ring to 1024 bytes"""
+    src = _src("gemm_ws.cu")
+    for rule in ("constexpr int kTileBytes = BM * BK * 2;",
+                 "template <int kBN> constexpr int kStageBytes = kTileBytes + kBN * BK * 2;",
+                 "template <int kBN> constexpr int kStagingBytes = BM * kBN * 2;",
+                 "template <int kBN> constexpr int kSmemBytes = kStages * kStageBytes<kBN> + 2 * kStagingBytes<kBN> + 1024;"):
+        assert rule in src, f"gemm_ws.cu no longer contains {rule!r}: update the model"
+    stages = int(re.search(r"constexpr int kStages = (\d+);", src).group(1))
+    stage = 128 * 64 * 2 + bn * 64 * 2
+    assert stage % 1024 == 0, "a stage must keep the next one on the 1024-byte sw128 alignment"
+    return stages * stage + 2 * 128 * bn * 2 + 1024
 
 
 def linear_ws_schedule(tiles: int, sms: int, off_by_one: bool = False):
@@ -590,7 +677,9 @@ def conv_ws_rules():
                  "tma_load_4d(sA(s), &P.ta, bar, c0, bx + kx, by, bn);", "if ((c0 += BK) == p.Cin) {",
                  "if (++kx == P.taps_w) kx = 0, ++by;"):
         assert rule in s, f"gemm_ws.cu no longer contains {rule!r}: update the model"
-    assert "if (conv_ws_box(p, box)) return gemm_conv_ws(p, box, static_cast<int>(tiles), stream);" in _src("gemm_wgmma.cu")
+    for rule in ("const bool ws = p.mode == AV2V_A_LINEAR || conv_ws_box(p, box);",
+                 "if (ws) return gemm_conv_ws(p, box, static_cast<int>(tiles), stream);"):
+        assert rule in _src("gemm_wgmma.cu"), f"gemm_wgmma.cu no longer contains {rule!r}: update the model"
     return True
 
 
