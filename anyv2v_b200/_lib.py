@@ -62,6 +62,12 @@ class TAttnFusedArgs(Structure):
                 ("F", c_int32), ("HW", c_int32), ("heads", c_int32), ("Cx", c_int32), ("scale", c_float), ("n_v", c_int32)]
 
 
+class TAttnFusedQkSrcArgs(Structure):
+    _fields_ = [("x", c_void_p), ("qk_src", c_void_p), ("wqkv", c_void_p), ("o", c_void_p), ("ldx", c_int32),
+                ("ld_src", c_int32), ("ldo", c_int32), ("clips", c_int32), ("F", c_int32), ("HW", c_int32),
+                ("heads", c_int32), ("Cx", c_int32), ("scale", c_float)]
+
+
 class FreeUArgs(Structure):
     _fields_ = [("hidden", c_void_p), ("skip", c_void_p), ("out", c_void_p), ("NF", c_int32), ("H", c_int32), ("W", c_int32),
                 ("Ch", c_int32), ("Cs", c_int32), ("b", c_float), ("s", c_float)]
@@ -87,10 +93,12 @@ EXPORTS = {
     "av2v_ddim_step_eta_f16": (c_int, [POINTER(DdimEtaArgs), c_void_p]),
     "av2v_groupnorm_workspace_floats": (c_int, [c_int, c_int]),
     "av2v_groupnorm_silu_f16": (c_int, [POINTER(GroupNormArgs), c_void_p]),
+    "av2v_groupnorm_silu_part_f16": (c_int, [POINTER(GroupNormArgs), c_int32, c_void_p]),
     "av2v_gemm_f16": (c_int, [POINTER(GemmArgs), c_void_p]),
     "av2v_layernorm_f16": (c_int, [POINTER(LayerNormArgs), c_void_p]),
     "av2v_attn_pnp_f16": (c_int, [POINTER(AttnArgs), c_void_p]),
     "av2v_tattn_fused_f16": (c_int, [POINTER(TAttnFusedArgs), c_void_p]),
+    "av2v_tattn_fused_qksrc_f16": (c_int, [POINTER(TAttnFusedQkSrcArgs), c_void_p]),
     "av2v_freeu_f16": (c_int, [POINTER(FreeUArgs), c_void_p]),
     "av2v_tile_stitch_f16": (c_int, [POINTER(TileStitchArgs), c_void_p]),
 }

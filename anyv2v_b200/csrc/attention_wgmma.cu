@@ -6,7 +6,7 @@
 // (running max / sum per row, base-2 exponentials; a quarter of them on the FMA pipe, ex2_poly), converts P to fp16 in
 // registers — the accumulator layout of S is the A-fragment layout of the next wgmma — and accumulates O += P V with V read
 // MN-major ([keys][64], 64 contiguous) from shared memory.  With n_v = 3 (injected step) ONE P feeds the V of all three
-// branches.  K / V tiles are double-buffered with cp.async.  Rows-mode calls with 512 keys or more run attn_rows_kernel
+// branches; n_v = 2 is the same step replayed from cached source Q / K, the two edit branches only.  K / V tiles are double-buffered with cp.async.  Rows-mode calls with 512 keys or more run attn_rows_kernel
 // instead: the same per-row algorithm, warp-specialized (ring.cuh).  av2v_tattn_fused_f16 runs tattn_fused_kernel:
 // persistent, its Q/K/V projection fed through the same ring, then the same attention per item (see its comment below).
 //
@@ -261,7 +261,8 @@ constexpr int attn_smem() { return 2 * kTile + 2 * (1 + NV) * kTile + 1024; }
 // keys past seq_kv and query rows past seq, so 0 * NaN never reaches PV.  Per turn a consumer issues PV(j) and S(j + 1)
 // as one wgmma group, hands over, waits for it, releases stage j and runs softmax(j + 1) under the other's MMAs.
 // Key tile: 128 keys at NV = 1 (S m64n128, half the rescale work of 64); 64 at NV = 3, where O alone holds 96 registers and
-// S + P of 128 keys would not fit the 168 a thread of a 384-thread CTA is compiled for.
+// S + P of 128 keys would not fit the 168 a thread of a 384-thread CTA is compiled for.  NV = 2 keeps the 64 keys of NV = 3:
+// a branch's online softmax then rescales at the same tiles, so its output is bit-identical to the same branch at NV = 3.
 // Per-row algorithm as attn_tile: running max over raw scores, x = s * scale_log2 - ref in one FMA, a quarter of the
 // exponentials (key columns 24-31 of every 32) on the FMA pipe, fp16 P as the register A operand of PV, one division by l at
 // the store.
@@ -458,8 +459,11 @@ __global__ void __launch_bounds__(kRowsThreads, 1) attn_rows_kernel(const __grid
 // slots (after the other warpgroup has finished the previous item's attention: named barrier 1), and after a second barrier
 // runs the attention of its 64 slots against the keys of the same pixel and stores O.  Each accumulator sums its K blocks in
 // order, one wgmma group at a time, so results do not depend on the ring depth, the schedule or the grid size.
+// QK = true (av2v_tattn_fused_qksrc_f16, NV = 2): pass 0 projects Q and K alone from the source tensor (map tqk, same box), and
+// NV V-only passes follow, one per edit clip.  Every accumulator sums the same K blocks in the same order as at NV = 3.
 struct TAttnP {
-  CUtensorMap tx;  // x as (channel, frame, pixel, clip), box {64, F, ppt, 1}
+  CUtensorMap tx;   // x as (channel, frame, pixel, clip), box {64, F, ppt, 1}
+  CUtensorMap tqk;  // QK only: the Q / K source, same view and box
   CUtensorMap tw;  // wqkv [3C][Cx], box 64 x 64
   __half* o;
   int ldo, F, HW, heads, Cx, ppt, pix_tiles, src_clips, items;
@@ -485,9 +489,10 @@ __device__ __forceinline__ void acc_to_tile(const float (&acc)[32], uint32_t til
   }
 }
 
-template <int NV>
+template <int NV, bool QK = false>
 __global__ void __launch_bounds__(kTThreads, 1) tattn_fused_kernel(const __grid_constant__ TAttnP p) {
   constexpr int S = tattn_stages<NV>();
+  constexpr int passes = QK ? NV + 1 : NV;
   extern __shared__ uint8_t smem_raw[];
   __shared__ StageRing<S> ring;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -528,15 +533,19 @@ __global__ void __launch_bounds__(kTThreads, 1) tattn_fused_kernel(const __grid_
       for (int item = blockIdx.x; item < p.items; item += gridDim.x) {
         int h, pix0, clip;
         decode(item, h, pix0, clip);
-        // pass 0: Q, K, V of the (source) clip; pass b > 0: V of clip + b * src_clips
-        for (int b = 0; b < NV; ++b)
+        // pass 0: Q, K, V of the (source) clip; pass b > 0: V of clip + b * src_clips.  QK: pass 0 is Q, K of source clip
+        // `clip`, pass b > 0 the V of clip + (b - 1) * src_clips of x
+        constexpr int w0 = QK ? 2 : 3;  // weight boxes of pass 0
+        for (int b = 0; b < passes; ++b)
           for (int kb = 0; kb < nk; ++kb, ++g) {
             const int s = ring.stage(g);
-            uint64_t* bar = ring.produce(g, x_bytes + (b == 0 ? 3 : 1) * kTile);
-            tma_load_4d(sX(s), &p.tx, bar, kb * 64, 0, pix0, clip + b * p.src_clips);
+            uint64_t* bar = ring.produce(g, x_bytes + (b == 0 ? w0 : 1) * kTile);
+            if (!QK) tma_load_4d(sX(s), &p.tx, bar, kb * 64, 0, pix0, clip + b * p.src_clips);
+            else if (b == 0) tma_load_4d(sX(s), &p.tqk, bar, kb * 64, 0, pix0, clip);
+            else tma_load_4d(sX(s), &p.tx, bar, kb * 64, 0, pix0, clip + (b - 1) * p.src_clips);
             if (b == 0) {
 #pragma unroll
-              for (int q = 0; q < 3; ++q) tma_load_4d(sW(s, q), &p.tw, bar, kb * 64, q * C + h * HD, 0, 0);
+              for (int q = 0; q < w0; ++q) tma_load_4d(sW(s, q), &p.tw, bar, kb * 64, q * C + h * HD, 0, 0);
             } else {
               tma_load_4d(sW(s, 0), &p.tw, bar, kb * 64, 2 * C + h * HD, 0, 0);
             }
@@ -585,16 +594,16 @@ __global__ void __launch_bounds__(kTThreads, 1) tattn_fused_kernel(const __grid_
     decode(item, h, pix0, clip);
     const int pix_end = min(pix0 + p.ppt, p.HW);
     {
-      float acc[3][32];
+      float acc[QK ? 2 : 3][32];
       project(acc);
       // the other warpgroup has finished the previous item's attention (its reads of Q / K / V)
       if (item != blockIdx.x) named_bar_sync(1, 256);
       acc_to_tile(acc[0], sQ, wg);
       acc_to_tile(acc[1], sK, wg);
-      acc_to_tile(acc[2], sV(0), wg);
+      if constexpr (!QK) acc_to_tile(acc[2], sV(0), wg);
     }
 #pragma unroll
-    for (int b = 1; b < NV; ++b) {
+    for (int b = QK ? 0 : 1; b < NV; ++b) {
       float acc[1][32];
       project(acc);
       acc_to_tile(acc[0], sV(b), wg);
@@ -646,7 +655,7 @@ extern "C" int av2v_attn_pnp_f16(const av2v_attn_args* a, av2v_stream_t stream_)
   AV2V_REQUIRE(a != nullptr, AV2V_EINVAL, "attn: null args");
   AV2V_REQUIRE(a->q && a->k && a->v && a->o, AV2V_EINVAL, "attn: null q/k/v/o");
   AV2V_REQUIRE(a->batch > 0 && a->seq > 0 && a->heads > 0, AV2V_EINVAL, "attn: batch/seq/heads must be positive");
-  AV2V_REQUIRE(a->n_v == 1 || a->n_v == 3, AV2V_EINVAL, "attn: n_v must be 1 or 3 (got %d)", a->n_v);
+  AV2V_REQUIRE(a->n_v >= 1 && a->n_v <= 3, AV2V_EINVAL, "attn: n_v must be 1, 2 or 3 (got %d)", a->n_v);
   AV2V_REQUIRE(a->ldq % 8 == 0 && a->ldk % 8 == 0 && a->ldv % 8 == 0 && a->ldo % 8 == 0, AV2V_EALIGN,
                "attn: row strides must be multiples of 8 elements");
   AV2V_REQUIRE(a->ldq >= a->heads * HD && a->ldk >= a->heads * HD && a->ldv >= a->heads * HD &&
@@ -669,8 +678,8 @@ extern "C" int av2v_attn_pnp_f16(const av2v_attn_args* a, av2v_stream_t stream_)
   p.ldv = a->ldv;
   p.ldo = a->ldo;
   p.heads = a->heads;
-  p.v_branch_stride = a->n_v == 3 ? a->v_branch_stride : 0;
-  p.o_branch_stride = a->n_v == 3 ? a->o_branch_stride : 0;
+  p.v_branch_stride = a->n_v > 1 ? a->v_branch_stride : 0;
+  p.o_branch_stride = a->n_v > 1 ? a->o_branch_stride : 0;
   p.scale_log2 = a->scale * 1.4426950408889634f;
   p.seq = a->seq;
   p.seq_kv = a->seq_kv > 0 ? a->seq_kv : a->seq;
@@ -703,15 +712,17 @@ extern "C" int av2v_attn_pnp_f16(const av2v_attn_args* a, av2v_stream_t stream_)
   static bool attr_set = false;
   if (!attr_set) {
     AV2V_CHECK_CUDA(cudaFuncSetAttribute(attn_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn_smem<1>()));
+    AV2V_CHECK_CUDA(cudaFuncSetAttribute(attn_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn_smem<2>()));
     AV2V_CHECK_CUDA(cudaFuncSetAttribute(attn_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, attn_smem<3>()));
     AV2V_CHECK_CUDA(cudaFuncSetAttribute(attn_rows_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, rows_smem<1>()));
+    AV2V_CHECK_CUDA(cudaFuncSetAttribute(attn_rows_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, rows_smem<2>()));
     AV2V_CHECK_CUDA(cudaFuncSetAttribute(attn_rows_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, rows_smem<3>()));
     attr_set = true;
   }
   if (a->seq_mode == AV2V_SEQ_ROWS && p.seq_kv >= kRowsMinKeys) {
     AttnRowsP r{};
     const int C = a->heads * HD, kv_seqs = a->batch / p.kv_div;
-    const int kt = a->n_v == 3 ? rows_keys<3>() : rows_keys<1>();
+    const int kt = a->n_v == 1 ? rows_keys<1>() : a->n_v == 2 ? rows_keys<2>() : rows_keys<3>();
     if (int e = encode_rows_map(&r.tq, a->q, C, a->seq, a->batch, 1, a->ldq, 0, 128)) return e;
     if (int e = encode_rows_map(&r.tk, a->k, C, p.seq_kv, kv_seqs, 1, a->ldk, 0, kt)) return e;
     if (int e = encode_rows_map(&r.tv, a->v, C, p.seq_kv, kv_seqs, a->n_v, a->ldv, p.v_branch_stride, kt)) return e;
@@ -725,9 +736,56 @@ extern "C" int av2v_attn_pnp_f16(const av2v_attn_args* a, av2v_stream_t stream_)
     r.o_branch_stride = p.o_branch_stride;
     r.scale_log2 = p.scale_log2;
     if (a->n_v == 3) attn_rows_kernel<3><<<static_cast<unsigned>(items), kRowsThreads, rows_smem<3>(), stream>>>(r);
+    else if (a->n_v == 2) attn_rows_kernel<2><<<static_cast<unsigned>(items), kRowsThreads, rows_smem<2>(), stream>>>(r);
     else attn_rows_kernel<1><<<static_cast<unsigned>(items), kRowsThreads, rows_smem<1>(), stream>>>(r);
   } else if (a->n_v == 3) attn_kernel<3><<<static_cast<unsigned>(items), kThreads, attn_smem<3>(), stream>>>(p);
+  else if (a->n_v == 2) attn_kernel<2><<<static_cast<unsigned>(items), kThreads, attn_smem<2>(), stream>>>(p);
   else attn_kernel<1><<<static_cast<unsigned>(items), kThreads, attn_smem<1>(), stream>>>(p);
+  AV2V_CHECK_CUDA(cudaGetLastError());
+  return AV2V_OK;
+}
+
+// the launch of tattn_fused_kernel for validated arguments: a->n_v = 1 | 3, or n_v = 2 with Q / K from qk_src (QK = true)
+static int tattn_fused_launch(const av2v_tattn_fused_args* a, const void* qk_src, int ld_src, cudaStream_t stream) {
+  TAttnP p{};
+  p.o = static_cast<__half*>(a->o);
+  p.ldo = a->ldo;
+  p.F = a->F;
+  p.HW = a->HW;
+  p.heads = a->heads;
+  p.Cx = a->Cx;
+  p.ppt = 128 / a->F;
+  p.pix_tiles = (a->HW + p.ppt - 1) / p.ppt;
+  p.n_kt = 64 % a->F == 0 ? 1 : 2;
+  p.src_clips = a->n_v > 1 ? a->clips / a->n_v : a->clips;
+  p.scale_log2 = a->scale * 1.4426950408889634f;
+  const long long items = static_cast<long long>(p.src_clips) * a->heads * p.pix_tiles;
+  AV2V_REQUIRE(items < (1ll << 31), AV2V_ENOSUP, "tattn_fused: too many work items");
+  p.items = static_cast<int>(items);
+  // x [clips][F][HW][ldx] as (channel, frame, pixel, clip): the box {64, F, ppt, 1} lands in slot order (pixel-major)
+  auto x_map = [&](CUtensorMap* map, const void* base, int ld, int clips) {
+    const unsigned long long row = static_cast<unsigned long long>(ld) * 2, frame = row * a->HW;
+    const unsigned long long dims[4] = {static_cast<unsigned long long>(a->Cx), static_cast<unsigned long long>(a->F),
+                                        static_cast<unsigned long long>(a->HW), static_cast<unsigned long long>(clips)};
+    const unsigned long long strides[3] = {frame, row, frame * a->F};
+    const unsigned box[4] = {64, static_cast<unsigned>(a->F), static_cast<unsigned>(p.ppt), 1};
+    return encode_map_4d(map, base, dims, strides, box);
+  };
+  if (int e = x_map(&p.tx, a->x, a->ldx, a->clips)) return e;
+  if (qk_src != nullptr)
+    if (int e = x_map(&p.tqk, qk_src, ld_src, p.src_clips)) return e;
+  if (int e = encode_rows_map(&p.tw, a->wqkv, a->Cx, 3 * a->heads * HD, 1, 1, a->Cx, 0, 64)) return e;
+  static bool attr_set = false;
+  if (!attr_set) {
+    AV2V_CHECK_CUDA(cudaFuncSetAttribute(tattn_fused_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, tattn_smem<1>()));
+    AV2V_CHECK_CUDA(cudaFuncSetAttribute(tattn_fused_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tattn_smem<2>()));
+    AV2V_CHECK_CUDA(cudaFuncSetAttribute(tattn_fused_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, tattn_smem<3>()));
+    attr_set = true;
+  }
+  const unsigned grid = static_cast<unsigned>(items < sm_count_cached() ? items : sm_count_cached());
+  if (qk_src != nullptr) tattn_fused_kernel<2, true><<<grid, kTThreads, tattn_smem<2>(), stream>>>(p);
+  else if (a->n_v == 3) tattn_fused_kernel<3><<<grid, kTThreads, tattn_smem<3>(), stream>>>(p);
+  else tattn_fused_kernel<1><<<grid, kTThreads, tattn_smem<1>(), stream>>>(p);
   AV2V_CHECK_CUDA(cudaGetLastError());
   return AV2V_OK;
 }
@@ -745,39 +803,23 @@ extern "C" int av2v_tattn_fused_f16(const av2v_tattn_fused_args* a, av2v_stream_
   AV2V_REQUIRE(a->scale > 0.f, AV2V_EINVAL, "tattn_fused: scale must be positive");
   AV2V_REQUIRE(a->n_v == 1 || a->n_v == 3, AV2V_EINVAL, "tattn_fused: n_v must be 1 or 3 (got %d)", a->n_v);
   AV2V_REQUIRE(a->n_v == 1 || a->clips % 3 == 0, AV2V_EINVAL, "tattn_fused: n_v = 3 needs clips = 3 x clips-per-branch (got %d)", a->clips);
+  return tattn_fused_launch(a, nullptr, 0, stream);
+}
 
-  TAttnP p{};
-  p.o = static_cast<__half*>(a->o);
-  p.ldo = a->ldo;
-  p.F = a->F;
-  p.HW = a->HW;
-  p.heads = a->heads;
-  p.Cx = a->Cx;
-  p.ppt = 128 / a->F;
-  p.pix_tiles = (a->HW + p.ppt - 1) / p.ppt;
-  p.n_kt = 64 % a->F == 0 ? 1 : 2;
-  p.src_clips = a->n_v == 3 ? a->clips / 3 : a->clips;
-  p.scale_log2 = a->scale * 1.4426950408889634f;
-  const long long items = static_cast<long long>(p.src_clips) * a->heads * p.pix_tiles;
-  AV2V_REQUIRE(items < (1ll << 31), AV2V_ENOSUP, "tattn_fused: too many work items");
-  p.items = static_cast<int>(items);
-  // x [clips][F][HW][ldx] as (channel, frame, pixel, clip): the box {64, F, ppt, 1} lands in slot order (pixel-major)
-  const unsigned long long row = static_cast<unsigned long long>(a->ldx) * 2, frame = row * a->HW;
-  const unsigned long long dims[4] = {static_cast<unsigned long long>(a->Cx), static_cast<unsigned long long>(a->F),
-                                      static_cast<unsigned long long>(a->HW), static_cast<unsigned long long>(a->clips)};
-  const unsigned long long strides[3] = {frame, row, frame * a->F};
-  const unsigned box[4] = {64, static_cast<unsigned>(a->F), static_cast<unsigned>(p.ppt), 1};
-  if (int e = encode_map_4d(&p.tx, a->x, dims, strides, box)) return e;
-  if (int e = encode_rows_map(&p.tw, a->wqkv, a->Cx, 3 * a->heads * HD, 1, 1, a->Cx, 0, 64)) return e;
-  static bool attr_set = false;
-  if (!attr_set) {
-    AV2V_CHECK_CUDA(cudaFuncSetAttribute(tattn_fused_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, tattn_smem<1>()));
-    AV2V_CHECK_CUDA(cudaFuncSetAttribute(tattn_fused_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, tattn_smem<3>()));
-    attr_set = true;
-  }
-  const unsigned grid = static_cast<unsigned>(items < sm_count_cached() ? items : sm_count_cached());
-  if (a->n_v == 3) tattn_fused_kernel<3><<<grid, kTThreads, tattn_smem<3>(), stream>>>(p);
-  else tattn_fused_kernel<1><<<grid, kTThreads, tattn_smem<1>(), stream>>>(p);
-  AV2V_CHECK_CUDA(cudaGetLastError());
-  return AV2V_OK;
+extern "C" int av2v_tattn_fused_qksrc_f16(const av2v_tattn_fused_qksrc_args* a, av2v_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  AV2V_REQUIRE(a != nullptr, AV2V_EINVAL, "tattn_fused_qksrc: null args");
+  AV2V_REQUIRE(a->x && a->qk_src && a->wqkv && a->o, AV2V_EINVAL, "tattn_fused_qksrc: null x / qk_src / wqkv / o");
+  AV2V_REQUIRE(a->clips > 0 && a->clips % 2 == 0 && a->F > 0 && a->HW > 0 && a->heads > 0 && a->Cx > 0, AV2V_EINVAL,
+               "tattn_fused_qksrc: bad shape (clips must be even)");
+  AV2V_REQUIRE(a->F <= 128, AV2V_ENOSUP, "tattn_fused_qksrc: F must be at most 128 (got %d)", a->F);
+  AV2V_REQUIRE(a->Cx % 64 == 0, AV2V_ENOSUP, "tattn_fused_qksrc: the input width must be a multiple of 64 (got %d)", a->Cx);
+  AV2V_REQUIRE(a->ldx % 8 == 0 && a->ldx >= a->Cx && a->ld_src % 8 == 0 && a->ld_src >= a->Cx && a->ldo % 8 == 0 &&
+                   a->ldo >= a->heads * HD,
+               AV2V_EINVAL, "tattn_fused_qksrc: row strides must be multiples of 8 covering the rows");
+  AV2V_REQUIRE(aligned16(a->x) && aligned16(a->qk_src) && aligned16(a->wqkv) && aligned16(a->o), AV2V_EALIGN,
+               "tattn_fused_qksrc: pointers must be 16-byte aligned");
+  AV2V_REQUIRE(a->scale > 0.f, AV2V_EINVAL, "tattn_fused_qksrc: scale must be positive");
+  const av2v_tattn_fused_args b{a->x, a->wqkv, a->o, a->ldx, a->ldo, a->clips, a->F, a->HW, a->heads, a->Cx, a->scale, 2};
+  return tattn_fused_launch(&b, a->qk_src, a->ld_src, stream);
 }

@@ -460,8 +460,9 @@ extern "C" int av2v_groupnorm_workspace_floats(int n_samples, int C) {
   return n_samples * kGnMaxSlices * kGnMaxGroups * 2;
 }
 
-extern "C" int av2v_groupnorm_silu_f16(const av2v_groupnorm_args* a, av2v_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+// partition_samples > 0: cut the samples into chunks and slices as for a call of that many samples (the per-sample statistics
+// depend only on the slices, so they are then those of that call)
+static int groupnorm_launch(const av2v_groupnorm_args* a, int partition_samples, cudaStream_t stream) {
   AV2V_REQUIRE(a != nullptr, AV2V_EINVAL, "groupnorm: null args");
   AV2V_REQUIRE(a->x && a->y && a->gamma && a->beta && a->workspace, AV2V_EINVAL, "groupnorm: null pointer");
   AV2V_REQUIRE(a->n_samples > 0 && a->rows > 0 && a->C > 0 && a->groups > 0, AV2V_EINVAL, "groupnorm: bad shape");
@@ -509,10 +510,11 @@ extern "C" int av2v_groupnorm_silu_f16(const av2v_groupnorm_args* a, av2v_stream
   const long long sample_bytes = static_cast<long long>(a->rows) * row_bytes;
   long long cs = kChunkBytes / sample_bytes;
   if (cs < 1) cs = 1;
-  if (cs > a->n_samples) cs = a->n_samples;
+  const int np = partition_samples > 0 ? partition_samples : a->n_samples;
+  if (cs > np) cs = np;
   // spread the samples evenly over the chunks (48 frames of 2.6 MB: 3 x 16, not 18 + 18 + 12)
-  const int n_chunks = static_cast<int>((a->n_samples + cs - 1) / cs);
-  p.chunk_samples = (a->n_samples + n_chunks - 1) / n_chunks;
+  const int n_chunks = static_cast<int>((np + cs - 1) / cs);
+  p.chunk_samples = (np + n_chunks - 1) / n_chunks;
   p.n_chunks = (a->n_samples + p.chunk_samples - 1) / p.chunk_samples;
 
   // slices per sample: the chunk's items (chunk_samples x slices) should fill whole rounds of the grid (one CTA per SM) — 48
@@ -554,4 +556,15 @@ extern "C" int av2v_groupnorm_silu_f16(const av2v_groupnorm_args* a, av2v_stream
   else gn_persistent_kernel<3, 640><<<grid, T + 32, smem, stream>>>(p);
   AV2V_CHECK_CUDA(cudaGetLastError());
   return AV2V_OK;
+}
+
+extern "C" int av2v_groupnorm_silu_f16(const av2v_groupnorm_args* a, av2v_stream_t stream) {
+  return groupnorm_launch(a, 0, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int av2v_groupnorm_silu_part_f16(const av2v_groupnorm_args* a, int32_t partition_samples,
+                                            av2v_stream_t stream) {
+  AV2V_REQUIRE(a != nullptr && partition_samples >= a->n_samples, AV2V_EINVAL,
+               "groupnorm: partition_samples must be at least n_samples");
+  return groupnorm_launch(a, partition_samples, static_cast<cudaStream_t>(stream));
 }

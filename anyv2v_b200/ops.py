@@ -173,9 +173,11 @@ def ddim_step_eta(x, v_neg, v_edit, noise, guidance: float, ca: float, cb: float
 
 
 # ----------------------------------------------------------------------------------------------------------- K6
-def groupnorm(x, gamma, beta, groups: int, eps: float, silu: bool, out=None, x2=None):
+def groupnorm(x, gamma, beta, groups: int, eps: float, silu: bool, out=None, x2=None, partition_samples: int = 0):
     """GroupNorm(+SiLU) over x[n_samples, rows, C] (channels-last). pnp_utils.py:48-49,92,104.
-    x2: second source — the logical input is [x | x2] along the channels (skip-concat without torch.cat); out is [n, rows, C1 + C2]."""
+    x2: second source — the logical input is [x | x2] along the channels (skip-concat without torch.cat); out is [n, rows, C1 + C2].
+    partition_samples (>= n_samples): reduce each sample as a call of that many samples would, so that its statistics are
+    bit for bit those of that call."""
     global _launches
     _f16_cuda(x, "groupnorm.x")
     assert x.dim() == 3 and x.is_contiguous()
@@ -201,7 +203,11 @@ def groupnorm(x, gamma, beta, groups: int, eps: float, silu: bool, out=None, x2=
         _gn_ws[key] = ws
     a = L.GroupNormArgs(_p(x), _p(out), _p(gamma), _p(beta), _p(ws), n, rows, C, groups, eps, 1 if silu else 0, _p(x2), C1)
     with _timed(f"groupnorm n={n} rows={rows} C={C}"):
-        L.check(L.lib().av2v_groupnorm_silu_f16(ctypes.byref(a), _stream()), "av2v_groupnorm_silu_f16")
+        if partition_samples:
+            L.check(L.lib().av2v_groupnorm_silu_part_f16(ctypes.byref(a), partition_samples, _stream()),
+                    "av2v_groupnorm_silu_part_f16")
+        else:
+            L.check(L.lib().av2v_groupnorm_silu_f16(ctypes.byref(a), _stream()), "av2v_groupnorm_silu_f16")
     _launches += 1
     return out
 
@@ -460,11 +466,14 @@ def attention(q, k, v, heads: int, seq: int, batch: int, out, scale: float = 0.1
               v_branch_stride: int = 0, o_branch_stride: int = 0, frames_mode: bool = False, HW: int = 0,
               seq_kv: int = 0, kv_batch_div: int = 0):
     """PnP self-attention core (pnp_utils.py:189-210 / 295-316). q,k,v,out: 2-D token matrices (row-strided views ok).
-    frames_mode: temporal attention over frame-major tokens [batch / HW clips][seq = F frames][HW][*]; any F >= 1."""
+    frames_mode: temporal attention over frame-major tokens [batch / HW clips][seq = F frames][HW][*]; any F >= 1.
+    n_v = 3: q, k of the source branch, V / out of [source, uncond, cond] at v / out + b * branch stride; n_v = 2: the same
+    with the two edit branches only (each bit-identical to the same branch at n_v = 3)."""
     global _launches
     for name, t in (("q", q), ("k", k), ("v", v), ("o", out)):
         _f16_cuda(t, "attention." + name)
         assert t.dim() == 2 and t.stride(1) == 1
+    _require(n_v in (1, 2, 3), f"attention: n_v must be 1, 2 or 3, got {n_v}")
     C, extra = heads * 64, n_v - 1
     kv_rows = batch * seq if frames_mode else batch // max(kv_batch_div, 1) * (seq_kv if seq_kv > 0 else seq)
     _reach(q, "attention.q", batch * seq, C)
@@ -499,5 +508,28 @@ def temporal_attention_fused(x, wqkv, heads: int, F: int, HW: int, clips: int, o
     a = L.TAttnFusedArgs(_p(x), _p(wqkv), _p(out), x.stride(0), out.stride(0), clips, F, HW, heads, x.shape[1], scale, n_v)
     with _timed(f"temporal attention fused nv={n_v} clips={clips} F={F} HW={HW} heads={heads} Cx={x.shape[1]}"):
         L.check(L.lib().av2v_tattn_fused_f16(ctypes.byref(a), _stream()), "av2v_tattn_fused_f16")
+    _launches += 1
+    return out
+
+
+def temporal_attention_fused_qksrc(x, qk_src, wqkv, heads: int, F: int, HW: int, clips: int, out, scale: float = 0.125):
+    """``temporal_attention_fused`` of a PnP-injected step with Q and K projected from ``qk_src`` (the source branch's tokens
+    cached by an earlier edit of the clip): x: the edit clips [uncond | cond], frame-major [clips*F*HW, Cx]; qk_src: the
+    clips / 2 source clips [clips/2*F*HW, Cx] (its own row stride); out: [clips*F*HW, heads*64].  Clip c + b * clips / 2
+    attends with the Q, K of source clip c; each clip's output is bit-identical to the same clip at n_v = 3."""
+    global _launches
+    for name, t in (("x", x), ("qk_src", qk_src), ("wqkv", wqkv), ("o", out)):
+        _f16_cuda(t, "temporal_attention_fused_qksrc." + name)
+        _require(t.dim() == 2 and t.stride(1) == 1, f"temporal_attention_fused_qksrc.{name}: expected a 2-D row-major matrix")
+    _require(wqkv.is_contiguous() and wqkv.shape[0] == 3 * heads * 64 and wqkv.shape[1] == x.shape[1] == qk_src.shape[1],
+             "temporal_attention_fused_qksrc: wqkv must be a contiguous [3*heads*64, Cx] matching x and qk_src")
+    _require(clips % 2 == 0 and x.shape[0] == clips * F * HW == out.shape[0] and qk_src.shape[0] == clips // 2 * F * HW,
+             f"temporal_attention_fused_qksrc: x / out need {clips} clips and qk_src {clips // 2} of {F} x {HW} tokens")
+    _require(out.shape[1] >= heads * 64, f"temporal_attention_fused_qksrc.o: {out.shape[1]} columns, the heads need {heads * 64}")
+    _require(x.device == qk_src.device == wqkv.device == out.device, "temporal_attention_fused_qksrc: tensors on different devices")
+    a = L.TAttnFusedQkSrcArgs(_p(x), _p(qk_src), _p(wqkv), _p(out), x.stride(0), qk_src.stride(0), out.stride(0), clips, F, HW,
+                              heads, x.shape[1], scale)
+    with _timed(f"temporal attention fused qksrc clips={clips} F={F} HW={HW} heads={heads} Cx={x.shape[1]}"):
+        L.check(L.lib().av2v_tattn_fused_qksrc_f16(ctypes.byref(a), _stream()), "av2v_tattn_fused_qksrc_f16")
     _launches += 1
     return out

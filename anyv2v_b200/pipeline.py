@@ -27,8 +27,9 @@ from typing import Callable, Optional
 import torch
 
 from .latent_store import LatentStore
-from .pnp_utils import _fires, register_time
+from .pnp_utils import _PNP_SITES, _fires, register_time
 from .schedulers import randn_tensor
+from .unet_i2vgen_xl import SourceFeature
 
 logger = logging.getLogger(__name__)
 
@@ -86,6 +87,108 @@ def _loop_state(latents, timesteps, scheduler, guidance_scale: float, device, et
     st.iterations = {}  # graph key of the loop -> _GraphedIteration
     st.graph_pool = torch.cuda.graph_pool_handle() if st.latents.is_cuda else None
     return st
+
+
+def _pnp_sites(unet):
+    """[(name, site)] of the 17 PnP injection sites: the conv-injected resnet, then the spatial and the temporal attn1
+    processors of up_blocks[1..3] (pnp_utils.py:130, 235, 340)"""
+    sites = [("conv", unet.up_blocks[1].resnets[1])]
+    for kind, attr in (("spatial", "attentions"), ("temporal", "temp_attentions")):
+        for res, blocks in _PNP_SITES.items():
+            for blk in blocks:
+                sites.append((f"{kind}{res}.{blk}", getattr(unet.up_blocks[res], attr)[blk].transformer_blocks[0].attn1.processor))
+    return sites
+
+
+class SourceFeatureCache:
+    """The source branch's features at the PnP injection sites, kept from one edit of an inverted clip for the later edits of
+    the same clip (``I2VGenXLPipeline.source_feature_cache``; ``sample_with_pnp(..., source_features=cache)``).
+
+    Branch 0 of the edit's [source, uncond, cond] batch runs the UNet on the stored inverted latents with the inversion's
+    prompt and first frame: nothing of it depends on the edit, and only its features at the firing injection sites are read.
+    An edit step whose (t, firing sites, FreeU state) the cache holds therefore runs the UNet on [uncond, cond] only, with the
+    injection sites fed from the cache; any other injected step runs the three branches as without the cache and stores its
+    source features, as long as they fit in ``max_bytes``.  Either way the edit's latents are bit-identical to those of the
+    same edit without the cache.  What the cache stores per site: the normed tokens at the spatial and temporal attn1 sites
+    (Q and K are re-projected from them), conv2's input at the conv site; about 430 MB for a step with all three injections
+    at 16 x 512 x 512, in proportion to frames x h x w.
+
+    The cache belongs to one clip and one inversion: its first edit records the latent store (or ``ddim_inv_latents_path``),
+    the inversion prompt, first-frame embeddings and latents, ``target_fps``, the latents' frames x h x w and the UNet, and
+    an edit that differs in any of them raises ValueError.  The edit prompt, the edited first frame, the injection schedules,
+    guidance and eta may change from edit to edit."""
+
+    def __init__(self, unet, max_bytes: int):
+        if max_bytes < 0:
+            raise ValueError(f"max_bytes must be >= 0, got {max_bytes}")
+        self.unet = unet
+        self.max_bytes = int(max_bytes)
+        self.nbytes = 0
+        self.entries = {}     # (t, firing sites, FreeU state) -> {site name: feature}
+        self.features = {}    # site name -> SourceFeature: the static buffers the (captured) steps read and write
+        self._identity = None
+
+    def __len__(self):
+        return len(self.entries)
+
+    def bind(self, store_id, prompt_embeds, image_embeddings, image_latents, target_fps, frames_hw, unet):
+        """records what the source branch is computed from on the first edit; raises ValueError when a later edit differs"""
+        tensors = (prompt_embeds, image_embeddings, image_latents)
+        if unet is not self.unet:
+            raise ValueError("source_features: the cache was made for another UNet")
+        if self._identity is None:
+            self._identity = (store_id, tuple(t.detach().clone() for t in tensors), int(target_fps), tuple(frames_hw))
+            return
+        sid, ref, fps, fhw = self._identity
+        same_store = sid[0] == store_id[0] and (sid[1] == store_id[1] if sid[0] == "path" else sid[1] is store_id[1])
+        if not same_store:
+            raise ValueError("source_features: the cache holds the features of another inversion (latent store / "
+                             "ddim_inv_latents_path differs)")
+        for name, a, b in zip(("ddim_inv_prompt_embeds", "ddim_inv_image_embeddings", "ddim_inv_image_latents"), ref, tensors):
+            if a.shape != b.shape or not torch.equal(a, b.to(device=a.device, dtype=a.dtype)) or a.dtype != b.dtype:
+                raise ValueError(f"source_features: `{name}` differs from the edit the cache was filled by")
+        if fps != int(target_fps):
+            raise ValueError(f"source_features: target_fps {target_fps} differs from the cache's {fps}")
+        if fhw != tuple(frames_hw):
+            raise ValueError(f"source_features: frames x h x w {tuple(frames_hw)} differs from the cache's {fhw}")
+
+    def _feature(self, name):
+        f = self.features.get(name)
+        if f is None:
+            f = self.features[name] = SourceFeature()
+        return f
+
+    def begin_step(self, key, sites):
+        """-> "replay" (the cache holds ``key``: its features are copied to the static buffers), "capture" (the firing sites
+        store their source features) or None (they would not fit); attaches the sites' features in that mode"""
+        firing = [name for (name, _), f in zip(sites, key[1]) if f]
+        entry = self.entries.get(key)
+        if entry is not None:
+            mode = "replay"
+            for name in firing:
+                self.features[name].buf.copy_(entry[name])
+        else:
+            known = [self.features[n].buf for n in firing if n in self.features and self.features[n].buf is not None]
+            need = sum(b.numel() * b.element_size() for b in known)
+            mode = "capture" if self.nbytes + need <= self.max_bytes else None
+        for name, site in sites:
+            feat = self._feature(name)
+            feat.mode = mode
+            site.source_feature = feat
+        return mode
+
+    def end_step(self, key, sites, mode):
+        """detaches the sites; after a capture, keeps the step's features if they fit"""
+        for _, site in sites:
+            site.source_feature = None
+        if mode != "capture":
+            return
+        firing = [name for (name, _), f in zip(sites, key[1]) if f]
+        bufs = {n: self.features[n].buf for n in firing}
+        need = sum(b.numel() * b.element_size() for b in bufs.values())
+        if self.nbytes + need <= self.max_bytes:
+            self.entries[key] = {n: b.clone() for n, b in bufs.items()}
+            self.nbytes += need
 
 
 def tensor2vid(video: torch.Tensor, output_type: str = "np"):
@@ -239,6 +342,13 @@ class I2VGenXLPipeline:
     def disable_vae_tiling(self):
         """Back to whole-frame encode and decode."""
         self._require_vae().disable_tiling()
+
+    def source_feature_cache(self, max_bytes: int) -> SourceFeatureCache:
+        """A cache of the source branch's injection-site features for several PnP edits of one inverted clip: pass it as
+        ``sample_with_pnp(..., source_features=cache)`` to every edit; after the first, the injected steps it holds run the UNet
+        on two branches instead of three, with bit-identical results.  ``max_bytes`` bounds its device memory (about 430 MB
+        per fully injected step at 16 x 512 x 512)."""
+        return SourceFeatureCache(self.unet, max_bytes)
 
     def register_modules(self, **kwargs):
         for k, v in kwargs.items():
@@ -502,11 +612,13 @@ class I2VGenXLPipeline:
                         ddim_inv_image_embeddings=None, ddim_inv_image_latents=None,
                         latent_store: Optional[LatentStore] = None, skip_dead_source_branch: bool = True,
                         callback: Optional[Callable] = None, max_steps: Optional[int] = None,
-                        decode_chunk_size: Optional[int] = None, **_ignored):
+                        decode_chunk_size: Optional[int] = None, source_features: Optional[SourceFeatureCache] = None,
+                        **_ignored):
         """PnP edit loop (pipeline :1131-1179) over the branches [source, uncond, cond]; `output_type` "latent" returns
         the latents, "pt" / "np" / "pil" decode them with the attached VAE (:1180-1194).  ``eta > 0`` edits stochastically:
         every step, dead-source steps included, adds sigma_t * z with z drawn from ``generator`` as diffusers' DDIMScheduler
-        draws it (:1126, :1173)."""
+        draws it (:1126, :1173).  ``source_features`` (``source_feature_cache()``): reuse the source branch's features of
+        earlier edits of the same inverted clip, and keep this edit's; the result does not change."""
         # raw inputs (the reference's only interface, :1014-1094) are encoded once per clip when encoders / VAE are attached;
         # the source first frame is cropped to the size of the edited one
         height, width = self._size_of(image, height, width)
@@ -520,16 +632,17 @@ class I2VGenXLPipeline:
         st = self.prepare_edit(latents, prompt_embeds, negative_prompt_embeds, ddim_inv_prompt_embeds, image_embeddings,
                                image_latents, ddim_inv_image_embeddings, ddim_inv_image_latents, target_fps,
                                num_inference_steps, guidance_scale, ddim_init_latents_t_idx, ddim_inv_latents_path,
-                               latent_store, skip_dead_source_branch, eta, generator)
+                               latent_store, skip_dead_source_branch, eta, generator, source_features)
         self._loop(st, self.edit_step, callback, max_steps)
         return self._output(st.latents, output_type, return_dict, decode_chunk_size)
 
     def prepare_edit(self, latents, prompt_embeds, negative_prompt_embeds, ddim_inv_prompt_embeds, image_embeddings,
                      image_latents, ddim_inv_image_embeddings, ddim_inv_image_latents, target_fps, num_inference_steps,
                      guidance_scale, ddim_init_latents_t_idx=0, ddim_inv_latents_path=None, latent_store=None,
-                     skip_dead_source_branch=True, eta=0.0, generator=None):
+                     skip_dead_source_branch=True, eta=0.0, generator=None, source_features=None):
         """Everything of ``sample_with_pnp`` that happens once per clip (pipeline :1014-1128).  ``eta > 0``: the step noise
-        is drawn from ``generator`` (one generator, or a list of one)."""
+        is drawn from ``generator`` (one generator, or a list of one).  ``source_features``: a SourceFeatureCache, checked
+        against this edit's source inputs."""
         self._guidance_scale = guidance_scale
         if not self.do_classifier_free_guidance:
             raise NotImplementedError("the PnP edit path runs with classifier-free guidance (cfg 9.0)")
@@ -547,15 +660,22 @@ class I2VGenXLPipeline:
         # path the caller names (the reference only knows `ddim_inv_latents_path`, pipeline :1134)
         if latent_store is not None:
             store = latent_store
+            # a store read from a directory is identified by the directory, one kept in memory by the object
+            store_id = (("path", os.path.abspath(store.output_dir)) if store.output_dir is not None else ("store", store))
         elif ddim_inv_latents_path is not None:
             mine = self.latent_store
             same = (mine is not None and mine.output_dir is not None
                     and os.path.abspath(mine.output_dir) == os.path.abspath(ddim_inv_latents_path))
             store = mine if same else LatentStore(ddim_inv_latents_path, write_files=False)
+            store_id = ("path", os.path.abspath(ddim_inv_latents_path))
         elif self.latent_store is not None:
             store = self.latent_store
+            store_id = (("path", os.path.abspath(store.output_dir)) if store.output_dir is not None else ("store", store))
         else:
             raise ValueError("need `latent_store` or `ddim_inv_latents_path`")
+        if source_features is not None:
+            source_features.bind(store_id, ddim_inv_prompt_embeds, ddim_inv_image_embeddings, ddim_inv_image_latents,
+                                 target_fps, (latents.shape[2], latents.shape[3], latents.shape[4]), self.unet)
         d = lambda x: x.to(dev)
         # [source, uncond, cond] stacks (:1043-1046, :1093-1101); uncond image embedding is zeros (:438)
         prompts3 = torch.cat([d(ddim_inv_prompt_embeds), d(negative_prompt_embeds), d(prompt_embeds)])
@@ -568,10 +688,11 @@ class I2VGenXLPipeline:
         logger.info("Sampling starts from latents_at_t=%s", ts[0] if ts else None)
         fires = [self._any_hook_fires(t) for t in ts]
         cond2 = None
-        if skip_dead_source_branch and not all(fires):
+        if (skip_dead_source_branch and not all(fires)) or source_features is not None:
             cond2 = {k: v[v.shape[0] // 3:].contiguous() for k, v in cond3.items()}  # every entry is branch-major
         st = _loop_state(latents, ts, self.scheduler, guidance_scale, dev, eta=float(eta), cond3=cond3, cond2=cond2, store=store,
-                         fires=fires, guidance=guidance_scale, skip=skip_dead_source_branch, generator=generator)
+                         fires=fires, guidance=guidance_scale, skip=skip_dead_source_branch, generator=generator,
+                         source_features=source_features)
         st.g_src = torch.zeros_like(st.latents)
         # uncond and cond are the same latents + image latents -> they share the UNet prefix up to the first cross-attention
         # (I2VGenXLUNet.forward, shared_edit_prefix); the source branch is dropped after the last injection site that fires in
@@ -611,12 +732,22 @@ class I2VGenXLPipeline:
         register_time(self, t)
         dead_source = st.skip and not st.fires[i]
         flags = self._hook_flags(t)
+        cache, mode = st.source_features, None
+        if cache is not None and st.fires[i]:
+            sites = _pnp_sites(self.unet)
+            cache_key = (t, tuple(_fires(t, getattr(s, "_injection_set", None)) for _, s in sites), self.unet.freeu_state())
+            mode = cache.begin_step(cache_key, sites)
+        two_branch = dead_source or mode == "replay"  # a replayed step injects into [uncond, cond] from the cache
 
         def make_body():
-            if dead_source:
+            if two_branch:
+                # a replayed step passes where the three-branch step would drop the source (_ReplayedSource)
+                replay = dict(source_replay=True, prune_source_after=self._prune_site(flags) if st.prune_source else None) \
+                    if mode == "replay" else {}
+
                 def body():
                     v = self.unet(torch.cat([st.latents, st.latents]), st.g_t, cond=st.cond2,
-                                  shared_edit_prefix=st.shared_prefix)[0]
+                                  shared_edit_prefix=st.shared_prefix, **replay)[0]
                     st.scheduler.step(v[0:1], None, st.latents, eta=st.eta, model_output_cond=v[1:2], out=st.latents,
                                       coef_dev=st.g_coef, variance_noise=st.g_noise)
                 return body
@@ -629,9 +760,18 @@ class I2VGenXLPipeline:
                 st.scheduler.step(v[lo:lo + 1], None, st.latents, eta=st.eta, model_output_cond=v[lo + 1:lo + 2],
                                   out=st.latents, coef_dev=st.g_coef, variance_noise=st.g_noise)
             return body
-        if not dead_source:
+        if not two_branch:
             st.g_src.copy_(st.store.get(t, device=st.latents.device), non_blocking=True)
         self._draw_noise(st)
-        # the eta = 0 keys are those of the loop without eta; eta > 0 is marked, as in call_step's key
-        key = (dead_source, flags, self.unet.freeu_state()) + ((True,) if st.eta > 0 else ())
-        return self._run(st, i, key, make_body)
+        # the eta = 0 keys are those of the loop without eta; eta > 0 is marked, as in call_step's key; so is a step that
+        # captures or replays source features
+        key = (dead_source, flags, self.unet.freeu_state()) + ((True,) if st.eta > 0 else ()) + ((mode,) if mode else ())
+        if cache is None or not st.fires[i]:
+            return self._run(st, i, key, make_body)
+        try:
+            out = self._run(st, i, key, make_body)
+        except BaseException:
+            cache.end_step(cache_key, sites, None)  # detach; keep nothing of a step that did not complete
+            raise
+        cache.end_step(cache_key, sites, mode)
+        return out

@@ -58,10 +58,15 @@ def register_conv_injection(model, injection_schedule):
     conv_module = model.unet.up_blocks[1].resnets[1]
 
     def forward(input_tensor, temb, scale: float = 1.0):
-        inject = _fires(getattr(conv_module, "t", None), conv_module._injection_set) and input_tensor.shape[0] % 3 == 0
-        if inject:
+        fire = _fires(getattr(conv_module, "t", None), conv_module._injection_set)
+        # a source feature in "replay" mode: the batch is [uncond, cond] and the source's conv2 input comes from the cache
+        source = getattr(conv_module, "source_feature", None) if fire else None
+        replay = source is not None and source.mode == "replay"
+        inject = fire and not replay and input_tensor.shape[0] % 3 == 0
+        if inject or replay:
             logger.debug("PnP Injecting Conv at t=%s", conv_module.t)
-        return to_nchw_view(conv_module.forward_nhwc(to_nhwc(input_tensor), temb, inject=inject))
+        return to_nchw_view(conv_module.forward_nhwc(to_nhwc(input_tensor), temb, inject=inject,
+                                                     source=source if inject or replay else None))
 
     conv_module.forward = forward
     setattr(conv_module, "injection_schedule", injection_schedule)

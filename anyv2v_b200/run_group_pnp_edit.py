@@ -111,7 +111,34 @@ def start_latents(pipe, ddim_scheduler, config, device):
     return mixed
 
 
-def edit_one(pipe, ddim_scheduler, config, device, rank_seed_offset: int = 0):
+def clip_key(config, rank_seed_offset: int = 0):
+    """what the source branch of an entry's edit is computed from, as the config names it: entries with equal keys edit the
+    same clip from the same inversion.  Synthetic entries draw their source stand-ins from their own seed."""
+    key = (config.ddim_latents_path, config.video_dir, config.video_name, tuple(config.image_size), config.n_frames,
+           config.target_fps, config.n_steps, config.seed, config.get("synthetic", False))
+    if config.get("synthetic", False):
+        return key + (rank_seed_offset,)
+    return key + (config.ddim_inv_prompt,)
+
+
+class SharedSourceFeatures:
+    """``share_source_features: true``: one SourceFeatureCache for consecutive entries of the same clip and inversion
+    (clip_key), dropped when the clip changes.  ``source_features_max_gb`` (default 24) bounds it."""
+
+    def __init__(self):
+        self.key, self.cache = None, None
+
+    def for_entry(self, pipe, config, rank_seed_offset: int = 0):
+        if not config.get("share_source_features", False):
+            return None
+        key = clip_key(config, rank_seed_offset)
+        if key != self.key:
+            self.cache = None  # the previous clip's features are released before the next ones are made
+            self.key, self.cache = key, pipe.source_feature_cache(int(float(config.get("source_features_max_gb", 24)) * 2**30))
+        return self.cache
+
+
+def edit_one(pipe, ddim_scheduler, config, device, rank_seed_offset: int = 0, source_features=None):
     config.video_path = os.path.join(config.video_dir, config.video_name + ".mp4")
     config.video_frames_path = os.path.join(config.video_dir, config.video_name)
     config.edited_first_frame_path = os.path.join(config.data_dir, config.edited_first_frame_path)
@@ -119,7 +146,7 @@ def edit_one(pipe, ddim_scheduler, config, device, rank_seed_offset: int = 0):
         if "ReplaceMe" in str(v):
             logger.error("Field %s contains 'ReplaceMe'", k)
     if not config.get("synthetic", False):
-        return edit_one_real(pipe, ddim_scheduler, config, device)
+        return edit_one_real(pipe, ddim_scheduler, config, device, source_features)
     h, w = config.image_size[1] // 8, config.image_size[0] // 8
     cross_dim = pipe.unet.config["cross_attention_dim"]
     cond = synthetic_conditioning(config.n_frames, h, w, cross_dim, config.seed + rank_seed_offset, device)
@@ -132,7 +159,7 @@ def edit_one(pipe, ddim_scheduler, config, device, rank_seed_offset: int = 0):
         ddim_inv_image_latents=cond["src_image_latents"], num_frames=config.n_frames,
         num_inference_steps=config.n_steps, guidance_scale=config.cfg, target_fps=config.target_fps,
         ddim_init_latents_t_idx=config.ddim_init_latents_t_idx, ddim_inv_latents_path=config.ddim_latents_path,
-        latent_store=store, output_type="latent").frames
+        latent_store=store, output_type="latent", source_features=source_features).frames
     output_dir = os.path.join(config.output_dir, config_suffix(config))
     os.makedirs(output_dir, exist_ok=True)
     torch.save(out.cpu(), os.path.join(output_dir, "edited_latents.pt"))
@@ -140,7 +167,7 @@ def edit_one(pipe, ddim_scheduler, config, device, rank_seed_offset: int = 0):
     return out
 
 
-def edit_one_real(pipe, ddim_scheduler, config, device):
+def edit_one_real(pipe, ddim_scheduler, config, device, source_features=None):
     """reference :95-183 on real inputs: frames + edited first frame + prompts -> edited video files."""
     from . import image_io
     Image = image_io._pil()
@@ -158,7 +185,7 @@ def edit_one_real(pipe, ddim_scheduler, config, device):
         target_fps=config.target_fps, latents=mixed, generator=torch.Generator(device=device).manual_seed(config.seed),
         return_dict=True, ddim_init_latents_t_idx=config.ddim_init_latents_t_idx,
         ddim_inv_latents_path=config.ddim_latents_path, ddim_inv_prompt=config.ddim_inv_prompt,
-        ddim_inv_1st_frame=src_1st_frame, output_type="latent").frames
+        ddim_inv_1st_frame=src_1st_frame, output_type="latent", source_features=source_features).frames
     video = pipe.decode_latents(latents)                                  # [1, 3, f, H, W] in [-1, 1]
     frames = image_io.frames_to_pil(video[0].permute(1, 0, 2, 3))
     output_dir = os.path.join(config.output_dir, config_suffix(config))
@@ -280,8 +307,10 @@ def run_sharded(build, template_config, configs_list, device, run_entry, unet_co
 
 def main(template_config, configs_list, device, unet_config=None, pipeline_kwargs=None):
     ddim_scheduler = DDIMScheduler.from_pretrained("ali-vilab/i2vgen-xl", subfolder="scheduler")
+    shared = SharedSourceFeatures()
     return run_sharded(build_pipeline, template_config, configs_list, device,
-                       lambda pipe, config, i: edit_one(pipe, ddim_scheduler, config, device, rank_seed_offset=i),
+                       lambda pipe, config, i: edit_one(pipe, ddim_scheduler, config, device, rank_seed_offset=i,
+                                                        source_features=shared.for_entry(pipe, config, i)),
                        unet_config, pipeline_kwargs)
 
 

@@ -113,10 +113,40 @@ class TemporalConv3(nn.Conv3d):
         return self._packed.get(self.weight, lambda w: w[:, :, :, 0, 0].permute(0, 2, 1).reshape(w.shape[0], -1))
 
 
+#: the _ReplayedSource of the UNet forward that is running, if it replays a PnP step from cached source features
+_replayed_source = None
+
+
 class GroupNorm(nn.GroupNorm):
     def forward_rows(self, x_rows: torch.Tensor, silu: bool, x2_rows: Optional[torch.Tensor] = None) -> torch.Tensor:
         """x_rows: [n_samples, rows, C] channels-last; with x2_rows the logical input is [x_rows | x2_rows] along the channels."""
-        return ops.groupnorm(x_rows, self.weight, self.bias, self.num_groups, self.eps, silu, x2=x2_rows)
+        part = _replayed_source.partition(x_rows.shape[0]) if _replayed_source is not None else 0
+        kw = {"partition_samples": part} if part else {}
+        return ops.groupnorm(x_rows, self.weight, self.bias, self.num_groups, self.eps, silu, x2=x2_rows, **kw)
+
+
+class SourceFeature:
+    """The source branch's feature at one PnP injection site, shared by the edits of one inverted clip
+    (pipeline.SourceFeatureCache): the normed tokens at an attention site, conv2's input at the conv site.  ``buf`` is the
+    site's static "current step" buffer, allocated on first use and then fixed, so that a captured step reads or writes
+    the same address every time.  mode "capture": the injected three-branch site also stores the source's feature into
+    ``buf``; "replay": the batch holds the two edit branches only and the site takes the source's feature from ``buf``."""
+    __slots__ = ("mode", "buf")
+
+    def __init__(self):
+        self.mode = None
+        self.buf = None
+
+    def keep(self, t: torch.Tensor) -> None:
+        if self.buf is None:
+            self.buf = torch.empty_like(t, memory_format=torch.contiguous_format)
+        self.buf.copy_(t)
+
+
+def _source_feature(site, mode: str):
+    """the SourceFeature attached to ``site`` (a PnP processor or the conv-injected resnet) when it is in ``mode``"""
+    feat = getattr(site, "source_feature", None)
+    return feat if feat is not None and feat.mode == mode else None
 
 
 # ------------------------------------------------------------------------------------------------ attention
@@ -158,11 +188,28 @@ class AttnProcessor:
             B = nb
         heads = attn.heads
         rows = tokens.shape[0]
-        inject = self.inject_now() and (B % 3 == 0)
+        fire = self.inject_now()
+        replay = _source_feature(self, "replay") if fire else None
+        inject = fire and replay is None and (B % 3 == 0)
+        capture = _source_feature(self, "capture") if inject else None
+        if capture is not None:
+            capture.keep(tokens[:rows // 3])                             # the source third's tokens
         wqkv = attn.fused_qkv_weight()
         out_attn = torch.empty((rows, C), dtype=tokens.dtype, device=tokens.device)
         fusable = frames_view and seq <= 128 and C % 64 == 0 and wqkv.shape[0] == 3 * heads * 64
-        if fusable:
+        if replay is not None:
+            # the injected step on [uncond, cond] with the source's tokens from the cache: Q, K projected from them as the
+            # injected branch below projects them, P applied to the V of the two edit branches
+            src_rows = rows // 2
+            if fusable:
+                ops.temporal_attention_fused_qksrc(tokens, replay.buf, wqkv, heads, seq, HW, B, out_attn, scale=attn.scale)
+            else:
+                qk = ops.linear(replay.buf, wqkv[:2 * C])
+                v = ops.linear(tokens, wqkv[2 * C:])
+                ops.attention(qk[:, :C], qk[:, C:], v, heads, seq, nbatch // 2, out_attn, scale=attn.scale, n_v=2,
+                              v_branch_stride=src_rows * C, o_branch_stride=src_rows * C, frames_mode=frames_view,
+                              HW=(HW if frames_view else 0))
+        elif fusable:
             # temporal self-attention: Q/K/V projection fused into the attention kernel (Q, K, V never reach HBM); on injected
             # steps (pnp_utils.py:295-302) Q and K of all three branches are projected from the SOURCE clip inside the kernel
             ops.temporal_attention_fused(tokens, wqkv, heads, seq, HW, B, out_attn, scale=attn.scale, n_v=3 if inject else 1)
@@ -191,17 +238,26 @@ class AttnProcessor:
     def _self_protocol_temporal(self, attn, x, residual):
         # [B*HW, F, C] contiguous: make it frame-major once (copy), run the fast path, convert back.
         nb, F, C = x.shape
-        xt = x.transpose(0, 1).contiguous().view(1, F, nb, C).permute(0, 2, 1, 3)  # [1, nb, F, C] frame-major view
+        fire = self.inject_now()
+        branches = 2 if fire and _source_feature(self, "replay") is not None else 3 if fire and nb % 3 == 0 else 0
+        if branches:
+            # keep branch-major grouping: [branches, nb/branches, F, C]
+            xt = x.view(branches, nb // branches, F, C).transpose(1, 2).contiguous().permute(0, 2, 1, 3)
+            rt = None if residual is None else residual.view(branches, nb // branches, F, C).transpose(1, 2).contiguous().permute(0, 2, 1, 3)
+            y = self._self(attn, xt, rt)  # [B', HW', F, C] view over frame-major memory
+            return y.reshape(nb, F, C).contiguous()  # back to the protocol layout [nb][F][C] (copy; short sequences only)
+        # a replayed step (_ReplayedSource) puts zero rows where the three-branch step has the source's sequences: the fused
+        # kernel packs the nb sequences as pixels of one clip, and a pixel's rounding depends on its place in the tile
+        pad = _replayed_source.pad(nb) if _replayed_source is not None else 0
+        if pad:
+            x = torch.cat([x.new_zeros(pad, F, C), x])
+            residual = None if residual is None else torch.cat([residual.new_zeros(pad, F, C), residual])
+        xt = x.transpose(0, 1).contiguous().view(1, F, nb + pad, C).permute(0, 2, 1, 3)  # [1, nb, F, C] frame-major view
         rt = None
         if residual is not None:
-            rt = residual.transpose(0, 1).contiguous().view(1, F, nb, C).permute(0, 2, 1, 3)
-        if self.inject_now() and nb % 3 == 0:
-            # keep branch-major grouping: [3, nb/3, F, C]
-            xt = x.view(3, nb // 3, F, C).transpose(1, 2).contiguous().permute(0, 2, 1, 3)
-            if residual is not None:
-                rt = residual.view(3, nb // 3, F, C).transpose(1, 2).contiguous().permute(0, 2, 1, 3)
+            rt = residual.transpose(0, 1).contiguous().view(1, F, nb + pad, C).permute(0, 2, 1, 3)
         y = self._self(attn, xt, rt)  # [B', HW', F, C] view over frame-major memory
-        return y.reshape(nb, F, C).contiguous()  # back to the protocol layout [nb][F][C] (copy; short sequences only)
+        return y.reshape(nb + pad, F, C)[pad:].contiguous()  # back to the protocol layout [nb][F][C] (copy; short sequences only)
 
     def _cross(self, attn, x, ctx, residual, kv_div: int = 1):
         """Cross-attention to the 145-token context.  ``ctx`` may hold ONE context per clip ([nb/kv_div, Nk, D]): the
@@ -442,18 +498,29 @@ class ResnetBlock2D(nn.Module):
         a2 = None if skip is None else skip.view(-1, cin - c1)
         return ops.linear(x.view(-1, c1), w2, bias=self.conv_shortcut.bias, a2=a2).view(nf, h, w, self.out_channels)
 
-    def forward_nhwc(self, x, temb, inject: bool = False, skip=None, temb_act=None):
+    def forward_nhwc(self, x, temb, inject: bool = False, skip=None, temb_act=None, source: Optional[SourceFeature] = None):
         """``skip`` (up blocks): the block's input is the channel concat [x | skip] (diffusers: torch.cat([hidden_states,
         res_hidden_states], dim=1)); it is never materialised — GroupNorm reads the two sources and writes the normalised
-        concat, the 1x1 shortcut runs its K loop over both.  ``temb_act`` = SiLU(temb), computed once per step by the caller."""
+        concat, the 1x1 shortcut runs its K loop over both.  ``temb_act`` = SiLU(temb), computed once per step by the caller.
+        ``source`` (PnP injection shared between edits): with ``inject``, mode "capture" keeps the source third's conv2 input;
+        mode "replay" (``inject`` off) runs the injected resnet on [uncond, cond] with that input taken from the cache."""
         nf, h, w, c1 = x.shape
         cin = self.in_channels
         hw = h * w
-        if skip is not None and (c1 % 64 != 0 or inject):
+        replay = source is not None and source.mode == "replay"
+        if skip is not None and (c1 % 64 != 0 or inject or replay):
             x, skip = torch.cat([x, skip], dim=-1), None   # widths the two-source K loop does not cover / the injected resnet
             c1 = cin
         if isinstance(temb, _Temb):
             temb, temb_act = temb.raw, temb.act
+        if replay:
+            # conv2 of the injected step's source third, from its cached input, stored to the two edit slots with their own
+            # shortcuts: the same tile and per-slot epilogue as the three-slot store below
+            n = nf // 2
+            short = self.shortcut_nhwc(x, skip)
+            out = torch.empty((nf, h, w, self.out_channels), dtype=x.dtype, device=x.device)
+            self.conv2.forward_nhwc(source.buf, residual=short, out=out, n_slots=2, slot_stride=n * hw * self.out_channels)
+            return out
         tproj = self.time_emb_proj(nr.silu(temb) if temb_act is None else temb_act)   # [NF, Cout]
         short = self.shortcut_nhwc(x, skip)
         if not inject:
@@ -470,6 +537,8 @@ class ResnetBlock2D(nn.Module):
         y = self.norm1.forward_rows(xs.reshape(n, hw, cin), silu=True).view(n, h, w, cin)
         y = self.conv1.forward_nhwc(y, rowbias=tproj[:n], rows_per_rowbias=hw)
         y = self.norm2.forward_rows(y.view(n, hw, -1), silu=True).view(n, h, w, -1)
+        if source is not None and source.mode == "capture":
+            source.keep(y)
         out = torch.empty((nf, h, w, self.out_channels), dtype=x.dtype, device=x.device)
         self.conv2.forward_nhwc(y, residual=short, out=out, n_slots=3, slot_stride=n * hw * self.out_channels)
         return out
@@ -556,6 +625,31 @@ class _SourcePrune:
         return (not self.done) and self.site == (block, layer, kind)
 
 
+class _ReplayedSource(_SourcePrune):
+    """``source_replay`` of I2VGenXLUNet.forward: the batch holds [uncond, cond] of a PnP step whose source branch's features come
+    from a cache; the step it stands for ran with the source branch present up to `site` (its prune site; None: to the end).
+    GroupNorm cuts a sample's reduction by the number of samples in the call, so up to that site every GroupNorm reduces as it
+    would with the source's samples there too (one branch more than ``present``): each sample's statistics, and so the edit
+    branches' results, are bit for bit those of the three-branch step.  Nothing is dropped at the site."""
+
+    def __init__(self, site, frames: int, present: int):
+        super().__init__(site if site is not None else (None, None, None), frames)
+        self.present = present
+
+    def frames(self, t):
+        return t
+
+    def clips(self, t):
+        return t
+
+    def partition(self, n: int) -> int:
+        return 0 if self.done else n + n // self.present
+
+    def pad(self, n: int) -> int:
+        """rows of the source branch in front of the n rows of the batch, in the three-branch step (0 after the site)"""
+        return 0 if self.done else n // self.present
+
+
 class _Block3D(nn.Module):
     def _layer(self, i, x, temb, ctx, nframes, prune=None, block_index=None, skip=None):
         """-> (x, temb, ctx); temb / ctx come back shortened when `prune` dropped the source branch inside this layer.
@@ -573,13 +667,15 @@ class _Block3D(nn.Module):
         x = self.temp_convs[i].forward_nhwc(x, nframes)
         if self.has_cross_attention:
             if prune is not None and prune.at(block_index, i, "spatial"):
-                temb, ctx, prune.done = prune.frames(temb), prune.clips(ctx), True
+                temb, ctx = prune.frames(temb), prune.clips(ctx)
                 x = self.attentions[i].forward_nhwc(x, ctx, expand=prune.frames)   # attn1 on all branches, the rest on the edit ones
+                prune.done = True                                                  # (after: its GroupNorm ran on all branches)
             else:
                 x = self.attentions[i].forward_nhwc(x, ctx)
             if prune is not None and prune.at(block_index, i, "temporal"):
-                temb, ctx, prune.done = prune.frames(temb), prune.clips(ctx), True
+                temb, ctx = prune.frames(temb), prune.clips(ctx)
                 x = self.temp_attentions[i].forward_nhwc(x, nframes, expand=prune.clips)
+                prune.done = True
             else:
                 x = self.temp_attentions[i].forward_nhwc(x, nframes)
         return x, temb, ctx
@@ -780,7 +876,25 @@ class I2VGenXLUNet(nn.Module):
 
     def forward(self, sample, timestep, fps=None, image_latents=None, image_embeddings=None,
                 encoder_hidden_states=None, cross_attention_kwargs=None, return_dict: bool = False, cond=None,
-                shared_edit_prefix: bool = False, prune_source_after=None):
+                shared_edit_prefix: bool = False, prune_source_after=None, source_replay: bool = False):
+        """See _forward.  ``source_replay`` (set by the PnP edit loop with a SourceFeatureCache): the batch is [uncond, cond] of an
+        injected step whose injection sites read the source branch's features from the cache; ``prune_source_after`` is then
+        where the three-branch step would have dropped the source (None: nowhere), and nothing is dropped (_ReplayedSource)."""
+        global _replayed_source
+        _replayed_source = None
+        if source_replay:
+            b, f, blk0 = sample.shape[0], sample.shape[2], self.down_blocks[0]
+            shared = (bool(shared_edit_prefix) and b >= 2 and blk0.has_cross_attention
+                      and "forward" not in blk0.resnets[0].__dict__)
+            _replayed_source = _ReplayedSource(prune_source_after, f, b - 1 if shared else b)
+        try:
+            return self._forward(sample, timestep, fps, image_latents, image_embeddings, encoder_hidden_states, cond,
+                                 shared_edit_prefix, None if source_replay else prune_source_after)
+        finally:
+            _replayed_source = None
+
+    def _forward(self, sample, timestep, fps, image_latents, image_embeddings, encoder_hidden_states, cond,
+                 shared_edit_prefix, prune_source_after):
         """Same call as pipeline_i2vgen_xl.py:1146-1155.  ``cond`` (optional) is precompute_conditioning()'s result.
 
         ``shared_edit_prefix`` (round-2 candidate, set by the PnP edit loop only): the caller guarantees that the LAST TWO
@@ -819,6 +933,8 @@ class I2VGenXLUNet(nn.Module):
             x = blk0.resnets[0].forward_nhwc(x, emb[:u * f])
             x = blk0.temp_convs[0].forward_nhwc(x, f)
             x = blk0.attentions[0].forward_nhwc(x, cond["ctx"], expand=expand)              # all b branches from here on
+            if _replayed_source is not None:
+                _replayed_source.present = b
             x = blk0.temp_attentions[0].forward_nhwc(x, f)
             skips.append(x)
             x, outs = blk0.forward_nhwc(x, emb, cond["ctx"], f, first_layer=1)
@@ -829,6 +945,8 @@ class I2VGenXLUNet(nn.Module):
             skips.extend(outs)
         x = self.mid_block.forward_nhwc(x, emb, cond["ctx"], f)
         prune = _SourcePrune(prune_source_after, f) if (prune_source_after is not None and b >= 2) else None
+        if _replayed_source is not None and _replayed_source.site != (None, None, None):
+            prune = _replayed_source
         ctx = cond["ctx"]
         for bi, blk in enumerate(self.up_blocks):
             x = blk.forward_nhwc(x, skips, emb, ctx, f, prune, bi)
@@ -836,7 +954,7 @@ class I2VGenXLUNet(nn.Module):
                 emb, ctx = prune.frames(emb), prune.clips(ctx)
         if prune is not None:
             assert prune.done, f"prune site {prune.site} was never reached"
-            b = b - 1
+            b = b - (prune is not _replayed_source)
         nf = b * f
         x = self.conv_norm_out.forward_rows(x.view(nf, h * w, -1), silu=True).view(nf, h, w, -1)
         x = self.conv_out.forward_nhwc(x)                                                    # [B*F, h, w, 4]

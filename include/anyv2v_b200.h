@@ -108,6 +108,10 @@ typedef struct {
   int32_t C1;      /* channels of x when x2 != NULL (multiple of 8) */
 } av2v_groupnorm_args;
 int av2v_groupnorm_silu_f16(const av2v_groupnorm_args* a, av2v_stream_t stream);
+/* The same with the samples cut into chunks and reduction slices as for a call of partition_samples (>= n_samples) samples.
+ * The statistics of a sample depend only on that cut, so a call on part of a batch gives each of its samples the
+ * statistics the call on the whole batch gives it (a PnP edit step replayed on two branches instead of three). */
+int av2v_groupnorm_silu_part_f16(const av2v_groupnorm_args* a, int32_t partition_samples, av2v_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * wgmma GEMM core:  out[slot][m, n] = sum_k A[m, k] * Wt[n, k] + bias[n] + rowbias[m / rows_per_rowbias, n]
@@ -179,7 +183,9 @@ int av2v_layernorm_f16(const av2v_layernorm_args* a, av2v_stream_t stream);
  *   - n_v = 1: plain attention for `batch` sequences.  n_v = 3 (injected step): q/k hold ONLY the source branch
  *     (`batch` = source sequences); the probabilities are computed once and applied to the V of the three
  *     branches (v + j*v_branch_stride), writing o + j*o_branch_stride — identical to the reference where
- *     q,k of uncond/cond are overwritten by the source's.
+ *     q,k of uncond/cond are overwritten by the source's.  n_v = 2 (injected step replayed from cached source
+ *     features): the same with V and o holding the two edit branches only; each branch's arithmetic is that of
+ *     the same branch at n_v = 3, so its output is bit-identical.
  *   - AV2V_SEQ_ROWS (spatial): sequence b = rows [b*seq, (b+1)*seq).
  *   - AV2V_SEQ_FRAMES (temporal): tokens live frame-major as [clips][F][HW][*]; sequence (clip, pixel) =
  *     rows clip*F*HW + f*HW + pixel, f = 0..F-1 (no [B,C,F,h,w]->[B*hw,F,C] transpose is materialised).
@@ -193,7 +199,7 @@ typedef struct {
   int32_t ldq, ldk, ldv, ldo;  /* row strides in elements, multiples of 8 */
   int32_t batch, seq, heads;   /* head_dim fixed at 64 */
   int32_t HW;                  /* AV2V_SEQ_FRAMES only */
-  int32_t n_v;                 /* 1 or 3 */
+  int32_t n_v;                 /* 1, 2 or 3 */
   int64_t v_branch_stride, o_branch_stride; /* elements */
   float scale;                 /* softmax scale (64^-0.5) */
   int32_t seq_kv;              /* AV2V_SEQ_ROWS: key/value sequence length (cross-attention); 0 = same as seq */
@@ -221,6 +227,20 @@ typedef struct {
   int32_t n_v;                 /* 1 | 3 */
 } av2v_tattn_fused_args;
 int av2v_tattn_fused_f16(const av2v_tattn_fused_args* a, av2v_stream_t stream);
+
+/* The injected temporal self-attention with Q and K projected from a separate source tensor (PnP edits that replay
+ * the source branch's features cached by an earlier edit of the same clip): qk_src holds the LayerNorm-ed source
+ * tokens frame-major as [clips / 2][F][HW][ld_src]; x holds the `clips` edit clips [uncond | cond] as above.  Q and K
+ * of clip c (and of clip c + clips / 2) come from source clip c, V from the clip itself.  Each edit clip's output is
+ * bit-identical to the same clip of the n_v = 3 call of av2v_tattn_fused_f16 whose source clip holds qk_src.
+ */
+typedef struct {
+  const void* x; const void* qk_src; const void* wqkv; void* o;
+  int32_t ldx, ld_src, ldo;    /* row strides in elements, multiples of 8 */
+  int32_t clips, F, HW, heads, Cx;  /* clips: of x, even */
+  float scale;
+} av2v_tattn_fused_qksrc_args;
+int av2v_tattn_fused_qksrc_f16(const av2v_tattn_fused_qksrc_args* a, av2v_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * FreeU at one skip connection of up_blocks[0] / up_blocks[1] (diffusers 0.26.3 `apply_freeu`, enabled through

@@ -902,3 +902,49 @@ def check_tattn_box_slots(F: int, HW: int, clips: int = 2, **kw):
         got = tattn_box_slots(F, HW, clips, clip, pt * ppt, **kw)
         assert (got == qrow).all(), f"F={F} HW={HW} clip {clip} tile {pt}: box slots differ from the slot map"
     return True
+
+
+def tattn_qksrc_constants():
+    """(stages, projection passes per item, empty-barrier arrivals) of tattn_fused_kernel<2, true> (av2v_tattn_fused_qksrc_f16),
+    as written in attention_wgmma.cu; also checks the pass order tattn_pass_sources restates"""
+    s = _src("attention_wgmma.cu")
+    k = kernel_body("attention_wgmma.cu", "tattn_fused_kernel")
+    m = re.search(r"tattn_stages\(\) \{ return NV == 1 \? (\d+) : (\d+); \}", s)
+    passes = re.search(r"constexpr int passes = QK \? NV \+ (\d+) : NV;", k)
+    arrivals = int(re.search(r"ring\.init\((\d+)\);", k).group(1))
+    for rule in ("for (int b = 0; b < passes; ++b)", "constexpr int w0 = QK ? 2 : 3;",
+                 "else if (b == 0) tma_load_4d(sX(s), &p.tqk, bar, kb * 64, 0, pix0, clip);",
+                 "else tma_load_4d(sX(s), &p.tx, bar, kb * 64, 0, pix0, clip + (b - 1) * p.src_clips);",
+                 "float acc[QK ? 2 : 3][32];", "for (int b = QK ? 0 : 1; b < NV; ++b) {"):
+        assert rule in k, f"tattn_fused_kernel no longer contains {rule!r}: update the model"
+    assert "tattn_fused_kernel<2, true><<<" in s, "av2v_tattn_fused_qksrc_f16 no longer launches tattn_fused_kernel<2, true>"
+    return int(m.group(2)), 2 + int(passes.group(1)), arrivals
+
+
+def tattn_pass_sources(nv: int, qk: bool, clip: int, src_clips: int, off_by_one: bool = False):
+    """[(tensor, clip, what)] of each projection pass of one item, in the kernel's order: without qk, pass 0 projects Q, K, V
+    of x's clip `clip` and pass b > 0 the V of clip + b * src_clips; with qk (n_v = 2), pass 0 projects Q, K of the source
+    tensor's clip `clip` and pass b > 0 the V of x's clip + (b - 1) * src_clips.  off_by_one: the V passes of the qk variant
+    read clip + b * src_clips (negative control)"""
+    if not qk:
+        return [("x", clip, "QKV")] + [("x", clip + b * src_clips, "V") for b in range(1, nv)]
+    d = 0 if off_by_one else 1
+    return [("src", clip, "QK")] + [("x", clip + (b - d) * src_clips, "V") for b in range(1, nv + 1)]
+
+
+def check_tattn_qksrc_passes(src_clips: int, **kw):
+    """every edit clip c + j * src_clips of x (j = 0, 1) has its V projected exactly once, by the item of source clip c, into
+    V branch j; Q / K come from the source tensor; the branches are those the n_v = 3 call gives to clips 1, 2 of [source |
+    uncond | cond]"""
+    seen = {}
+    for clip in range(src_clips):
+        passes = tattn_pass_sources(2, True, clip, src_clips, **kw)
+        assert passes[0] == ("src", clip, "QK")
+        three = tattn_pass_sources(3, False, clip, src_clips)
+        for j, (tensor, c, what) in enumerate(passes[1:]):
+            assert tensor == "x" and what == "V" and 0 <= c < 2 * src_clips, f"source clip {clip}: V pass {j} reads clip {c}"
+            assert c not in seen, f"edit clip {c} projected twice"
+            seen[c] = (clip, j)
+            assert three[1 + j][1] - src_clips == c, f"V branch {j} of source clip {clip} is not the n_v = 3 call's branch {j + 1}"
+    assert sorted(seen) == list(range(2 * src_clips))
+    return True
