@@ -29,6 +29,12 @@ class DdimEtaArgs(Structure):
                 ("cs", c_float), ("coef_dev", c_void_p)]
 
 
+class DpmArgs(Structure):
+    _fields_ = [("x", c_void_p), ("v_neg", c_void_p), ("v_edit", c_void_p), ("x0_prev", c_void_p), ("out", c_void_p),
+                ("n", c_int64), ("guidance", c_float), ("alpha", c_float), ("sigma", c_float), ("a", c_float), ("b", c_float),
+                ("c", c_float), ("coef_dev", c_void_p)]
+
+
 class GroupNormArgs(Structure):
     _fields_ = [("x", c_void_p), ("y", c_void_p), ("gamma", c_void_p), ("beta", c_void_p), ("workspace", c_void_p),
                 ("n_samples", c_int32), ("rows", c_int32), ("C", c_int32), ("groups", c_int32), ("eps", c_float),
@@ -91,6 +97,7 @@ EXPORTS = {
     "av2v_ddim_step_cfg_f16": (c_int, [POINTER(DdimArgs), c_void_p]),
     "av2v_ddim_inverse_step_f16": (c_int, [POINTER(DdimArgs), c_void_p]),
     "av2v_ddim_step_eta_f16": (c_int, [POINTER(DdimEtaArgs), c_void_p]),
+    "av2v_dpmpp2m_step_f16": (c_int, [POINTER(DpmArgs), c_void_p]),
     "av2v_groupnorm_workspace_floats": (c_int, [c_int, c_int]),
     "av2v_groupnorm_silu_f16": (c_int, [POINTER(GroupNormArgs), c_void_p]),
     "av2v_groupnorm_silu_part_f16": (c_int, [POINTER(GroupNormArgs), c_int32, c_void_p]),

@@ -1,4 +1,5 @@
-// HBM-bound row kernels of the hot path: fused CFG + DDIM step (K7, eta = 0 and eta > 0) and LayerNorm.  GroupNorm(+SiLU) (K6) is groupnorm.cu.
+// HBM-bound row kernels of the hot path: fused CFG + DDIM step (K7, eta = 0 and eta > 0), fused CFG + DPM-Solver++(2M) step
+// and LayerNorm.  GroupNorm(+SiLU) (K6) is groupnorm.cu.
 #include "host_util.cuh"
 #include "ptx.cuh"
 
@@ -109,6 +110,99 @@ int ddim_eta_launch(const av2v_ddim_eta_args* a, cudaStream_t stream) {
       static_cast<const __half*>(a->x), static_cast<const __half*>(a->v_neg), static_cast<const __half*>(a->v_edit),
       static_cast<const __half*>(a->noise), static_cast<__half*>(a->out), a->n, a->guidance, a->ca, a->cb, a->cc, a->cd,
       a->cs, a->coef_dev);
+  AV2V_CHECK_CUDA(cudaGetLastError());
+  return AV2V_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------- DPM-Solver++(2M)
+// One step t -> s of the multistep solver (anyv2v_b200/schedulers.py DPMSolverMultistepScheduler), v-prediction:
+//   v   = v_edit ? r16(v_neg + r16(g * r16(v_edit - v_neg))) : v_neg      (the CFG combine, rounded as ddim_one rounds it)
+//   x0  = r16(alpha * x - sigma * v)                                     (stored to x0_prev for the next step)
+//   D   = c != 0 ? x0 + c * (x0 - x0_prev) : x0                          (c = 0: first-order step; x0_prev is not read)
+//   out = r16(a * x + b * D)
+// Pinned rounding points: x0 and out are rounded to fp16 once each; everything between is fp32, one IEEE rounding per
+// operation in the order written (__fmul_rn / __fadd_rn / __fsub_rn, no FMA contraction), so a CPU restatement in fp32
+// tensor ops gives the same bits.  The kernel reads x0_prev before it overwrites the same element with x0.
+__device__ __forceinline__ void dpm_one(float x, float vn, float ve, float p, bool cfg, bool second, float g, float al,
+                                        float si, float a, float b, float c, float& x0_out, float& y_out) {
+  float v = vn;
+  if (cfg) {
+    const float d0 = r16(__fsub_rn(ve, vn));
+    const float d1 = r16(__fmul_rn(g, d0));
+    v = r16(__fadd_rn(vn, d1));
+  }
+  const float x0 = r16(__fsub_rn(__fmul_rn(al, x), __fmul_rn(si, v)));
+  const float d = second ? __fadd_rn(x0, __fmul_rn(c, __fsub_rn(x0, p))) : x0;
+  x0_out = x0;
+  y_out = __fadd_rn(__fmul_rn(a, x), __fmul_rn(b, d));
+}
+
+__global__ void __launch_bounds__(256)
+dpm_step_kernel(const __half* __restrict__ x, const __half* __restrict__ vn, const __half* __restrict__ ve,
+                __half* __restrict__ x0p, __half* __restrict__ out, long long n, float g, float al, float si, float a,
+                float b, float c, const float* __restrict__ coef_dev) {
+  if (coef_dev != nullptr) {
+    al = coef_dev[0];
+    si = coef_dev[1];
+    a = coef_dev[2];
+    b = coef_dev[3];
+    c = coef_dev[4];
+    g = coef_dev[5];
+  }
+  const bool cfg = ve != nullptr;
+  const bool second = c != 0.f;
+  const long long nvec = n >> 3;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < nvec; i += stride) {
+    const uint4 xv = reinterpret_cast<const uint4*>(x)[i];
+    const uint4 nv = reinterpret_cast<const uint4*>(vn)[i];
+    uint4 ev = nv;
+    if (cfg) ev = reinterpret_cast<const uint4*>(ve)[i];
+    uint4 pv = nv;
+    if (second) pv = reinterpret_cast<const uint4*>(x0p)[i];
+    const __half* xh = reinterpret_cast<const __half*>(&xv);
+    const __half* nh = reinterpret_cast<const __half*>(&nv);
+    const __half* eh = reinterpret_cast<const __half*>(&ev);
+    const __half* ph = reinterpret_cast<const __half*>(&pv);
+    uint4 ov, qv;
+    __half* oh = reinterpret_cast<__half*>(&ov);
+    __half* qh = reinterpret_cast<__half*>(&qv);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      float x0, y;
+      dpm_one(__half2float(xh[e]), __half2float(nh[e]), __half2float(eh[e]), __half2float(ph[e]), cfg, second, g, al, si, a,
+              b, c, x0, y);
+      qh[e] = __float2half_rn(x0);
+      oh[e] = __float2half_rn(y);
+    }
+    reinterpret_cast<uint4*>(x0p)[i] = qv;
+    reinterpret_cast<uint4*>(out)[i] = ov;
+  }
+  // tail (n not a multiple of 8)
+  const long long tail0 = nvec << 3;
+  for (long long i = tail0 + static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+    float x0, y;
+    dpm_one(__half2float(x[i]), __half2float(vn[i]), cfg ? __half2float(ve[i]) : 0.f, second ? __half2float(x0p[i]) : 0.f,
+            cfg, second, g, al, si, a, b, c, x0, y);
+    x0p[i] = __float2half_rn(x0);
+    out[i] = __float2half_rn(y);
+  }
+}
+
+int dpmpp2m_launch(const av2v_dpmpp2m_args* a, cudaStream_t stream) {
+  AV2V_REQUIRE(a != nullptr, AV2V_EINVAL, "dpmpp2m: null args");
+  AV2V_REQUIRE(a->n >= 0, AV2V_EINVAL, "dpmpp2m: negative element count");
+  if (a->n == 0) return AV2V_OK;
+  AV2V_REQUIRE(a->x && a->v_neg && a->x0_prev && a->out, AV2V_EINVAL, "dpmpp2m: null x / v_neg / x0_prev / out");
+  AV2V_REQUIRE(a->x0_prev != a->x && a->x0_prev != a->out && a->x0_prev != a->v_neg && a->x0_prev != a->v_edit,
+               AV2V_EINVAL, "dpmpp2m: x0_prev must not alias x / v_neg / v_edit / out");
+  AV2V_REQUIRE(aligned16(a->x) && aligned16(a->v_neg) && aligned16(a->x0_prev) && aligned16(a->out) &&
+                   (!a->v_edit || aligned16(a->v_edit)),
+               AV2V_EALIGN, "dpmpp2m: pointers must be 16-byte aligned");
+  dpm_step_kernel<<<ddim_blocks(a->n), 256, 0, stream>>>(
+      static_cast<const __half*>(a->x), static_cast<const __half*>(a->v_neg), static_cast<const __half*>(a->v_edit),
+      static_cast<__half*>(a->x0_prev), static_cast<__half*>(a->out), a->n, a->guidance, a->alpha, a->sigma, a->a, a->b,
+      a->c, a->coef_dev);
   AV2V_CHECK_CUDA(cudaGetLastError());
   return AV2V_OK;
 }
@@ -336,4 +430,7 @@ extern "C" int av2v_ddim_inverse_step_f16(const av2v_ddim_args* a, av2v_stream_t
 }
 extern "C" int av2v_ddim_step_eta_f16(const av2v_ddim_eta_args* a, av2v_stream_t stream) {
   return ddim_eta_launch(a, static_cast<cudaStream_t>(stream));
+}
+extern "C" int av2v_dpmpp2m_step_f16(const av2v_dpmpp2m_args* a, av2v_stream_t stream) {
+  return dpmpp2m_launch(a, static_cast<cudaStream_t>(stream));
 }

@@ -172,6 +172,48 @@ def ddim_step_eta(x, v_neg, v_edit, noise, guidance: float, ca: float, cb: float
     return out
 
 
+def _overlap(a: torch.Tensor, b: Optional[torch.Tensor]) -> bool:
+    """whether the byte ranges of two contiguous tensors intersect"""
+    if b is None or a.numel() == 0 or b.numel() == 0:
+        return False
+    a0, b0 = a.data_ptr(), b.data_ptr()
+    return a0 < b0 + b.numel() * b.element_size() and b0 < a0 + a.numel() * a.element_size()
+
+
+def dpmpp2m_step(x, v_neg, v_edit, x0_prev, guidance: float, alpha: float, sigma: float, a: float, b: float, c: float,
+                 out=None, coef_dev=None):
+    """Fused CFG + DPM-Solver++(2M) step (csrc/elementwise.cu dpm_step_kernel): x0 = alpha*x - sigma*v is written to
+    ``x0_prev`` (which holds the previous step's x0 on entry), out = a*x + b*(x0 + c*(x0 - x0_prev)).  ``out`` may be x;
+    ``x0_prev`` must not overlap any other operand.  ``coef_dev``: device {alpha, sigma, a, b, c, guidance}."""
+    global _launches
+    n = x.numel()
+    _vector(x, "dpmpp2m_step.x", n)
+    _vector(v_neg, "dpmpp2m_step.v_neg", n)
+    _vector(v_edit, "dpmpp2m_step.v_edit", n)
+    _f16_cuda(x0_prev, "dpmpp2m_step.x0_prev")
+    _vector(x0_prev, "dpmpp2m_step.x0_prev", n)
+    if out is None:
+        out = torch.empty_like(x)
+    _f16_cuda(out, "dpmpp2m_step.out")
+    _vector(out, "dpmpp2m_step.out", n)
+    for name, t in (("v_neg", v_neg), ("v_edit", v_edit), ("x0_prev", x0_prev), ("out", out)):
+        _require(t is None or t.device == x.device, f"dpmpp2m_step.{name}: on {t.device if t is not None else None}, x on {x.device}")
+    for name, t in (("x", x), ("v_neg", v_neg), ("v_edit", v_edit), ("out", out)):
+        _require(not _overlap(x0_prev, t), f"dpmpp2m_step.x0_prev overlaps {name}")
+    for name, t in (("v_neg", v_neg), ("v_edit", v_edit)):
+        _require(not _overlap(out, t), f"dpmpp2m_step.out overlaps {name} (only x may be updated in place)")
+    _require(out.data_ptr() == x.data_ptr() or not _overlap(out, x), "dpmpp2m_step.out partly overlaps x")
+    if coef_dev is not None:
+        _require(coef_dev.device == x.device and coef_dev.dtype == torch.float32 and coef_dev.numel() >= 6,
+                 f"dpmpp2m_step.coef_dev: expected >= 6 fp32 values on {x.device}, got {coef_dev.numel()} "
+                 f"{coef_dev.dtype} on {coef_dev.device}")
+    args = L.DpmArgs(_p(x), _p(v_neg), _p(v_edit), _p(x0_prev), _p(out), n, guidance, alpha, sigma, a, b, c, _p(coef_dev))
+    with _timed("dpmpp2m_step"):
+        L.check(L.lib().av2v_dpmpp2m_step_f16(ctypes.byref(args), _stream()), "av2v_dpmpp2m_step")
+    _launches += 1
+    return out
+
+
 # ----------------------------------------------------------------------------------------------------------- K6
 def groupnorm(x, gamma, beta, groups: int, eps: float, silu: bool, out=None, x2=None, partition_samples: int = 0):
     """GroupNorm(+SiLU) over x[n_samples, rows, C] (channels-last). pnp_utils.py:48-49,92,104.

@@ -76,7 +76,9 @@ def _loop_state(latents, timesteps, scheduler, guidance_scale: float, device, et
                 **fields) -> SimpleNamespace:
     """What the three sampling loops keep per clip: the latents the steps update in place (a copy: the captured graphs read
     this tensor for the life of the state), the per-step timestep / scheduler-coefficient tables, the static buffers the
-    step body reads them from, and the loop iterations (``I2VGenXLPipeline._run``) with their shared activation pool."""
+    step body reads them from, and the loop iterations (``I2VGenXLPipeline._run``) with their shared activation pool.  A
+    multistep scheduler (DPMSolverMultistepScheduler) also gets ``x0_prev``, the previous step's x0 that its step reads and
+    rewrites in place, allocated once so that the captured graphs keep its address; DDIM loops have none."""
     st = SimpleNamespace(latents=latents.to(device).contiguous().clone(), timesteps=timesteps, scheduler=scheduler, eta=eta,
                          **fields)
     st.t_table = torch.tensor(timesteps, device=device, dtype=torch.int64)
@@ -84,6 +86,7 @@ def _loop_state(latents, timesteps, scheduler, guidance_scale: float, device, et
     st.g_t = torch.zeros(1, device=device, dtype=torch.int64)
     st.g_coef = torch.zeros(st.coef_table.shape[-1], device=device, dtype=torch.float32)
     st.g_noise = torch.zeros_like(st.latents) if eta > 0 else None  # the step noise of eta > 0 (I2VGenXLPipeline._draw_noise)
+    st.x0_prev = torch.zeros_like(st.latents) if getattr(scheduler, "multistep", False) else None
     st.iterations = {}  # graph key of the loop -> _GraphedIteration
     st.graph_pool = torch.cuda.graph_pool_handle() if st.latents.is_cuda else None
     return st
@@ -426,7 +429,9 @@ class I2VGenXLPipeline:
         stochastically, drawing sigma_t * z from ``generator`` at every step as diffusers' DDIMScheduler does.  Raw inputs
         (``prompt`` strings, PIL ``image``) need ``encoders=`` and ``vae=``; pre-encoded ``prompt_embeds`` /
         ``negative_prompt_embeds`` / ``image_embeddings`` / ``image_latents`` (batch 1) are accepted instead.
-        ``output_type`` "latent" returns the latents [N, 4, F, h, w]; "pt" / "np" / "pil" decode them with the attached VAE."""
+        ``output_type`` "latent" returns the latents [N, 4, F, h, w]; "pt" / "np" / "pil" decode them with the attached VAE.
+        ``pipe.scheduler = DPMSolverMultistepScheduler.from_config(pipe.scheduler.config)`` samples with DPM-Solver++(2M)
+        (eta = 0 only), typically with half the steps."""
         if isinstance(prompt, list):
             if len(prompt) != 1:  # the reference builds its image latents per video, not per prompt (:797-802)
                 raise ValueError(f"one prompt per call (got {len(prompt)}): use num_videos_per_prompt for several videos")
@@ -502,12 +507,12 @@ class I2VGenXLPipeline:
             def body():
                 v = self.unet(torch.cat([st.latents, st.latents]), st.g_t, cond=st.cond, shared_edit_prefix=st.shared_prefix)[0]
                 st.scheduler.step(v[:n_videos], None, st.latents, eta=st.eta, model_output_cond=v[n_videos:], out=st.latents,
-                                  coef_dev=st.g_coef, variance_noise=st.g_noise)
+                                  coef_dev=st.g_coef, variance_noise=st.g_noise, x0_prev=st.x0_prev)
         else:
             def body():
                 v = self.unet(st.latents, st.g_t, cond=st.cond)[0]
                 st.scheduler.step(v, None, st.latents, eta=st.eta, out=st.latents, coef_dev=st.g_coef,
-                                  variance_noise=st.g_noise)
+                                  variance_noise=st.g_noise, x0_prev=st.x0_prev)
 
         st.body = body
         return st
@@ -559,6 +564,9 @@ class I2VGenXLPipeline:
         """Everything of ``invert`` that happens once per clip (pipeline :1316-1382).  With ``guidance_scale > 1`` the
         step runs the UNet on [uncond, cond] (:1387-1388: negative prompt, zero image embedding :420-422, same image
         latents :559-560) and combines them (:1407-1410) inside the fused inverse-DDIM kernel."""
+        if getattr(self.scheduler, "multistep", False):
+            raise ValueError(f"invert runs DDIM inversion: set `pipe.scheduler` to a DDIMInverseScheduler (got "
+                             f"{type(self.scheduler).__name__}; a multistep solver is for sampling and editing only)")
         self._guidance_scale = guidance_scale
         self.check_inputs(prompt_embeds, image_latents, image_embeddings, latents)
         cfg = self.do_classifier_free_guidance
@@ -618,7 +626,10 @@ class I2VGenXLPipeline:
         the latents, "pt" / "np" / "pil" decode them with the attached VAE (:1180-1194).  ``eta > 0`` edits stochastically:
         every step, dead-source steps included, adds sigma_t * z with z drawn from ``generator`` as diffusers' DDIMScheduler
         draws it (:1126, :1173).  ``source_features`` (``source_feature_cache()``): reuse the source branch's features of
-        earlier edits of the same inverted clip, and keep this edit's; the result does not change."""
+        earlier edits of the same inverted clip, and keep this edit's; the result does not change.  With a
+        ``DPMSolverMultistepScheduler`` as ``pipe.scheduler`` the edit takes DPM-Solver++(2M) steps (e.g. 25 instead of 50);
+        the inversion store must hold the source latents of each of its timesteps (a 50-step DDIM inversion holds those of
+        25 steps)."""
         # raw inputs (the reference's only interface, :1014-1094) are encoded once per clip when encoders / VAE are attached;
         # the source first frame is cropped to the size of the edited one
         height, width = self._size_of(image, height, width)
@@ -673,6 +684,15 @@ class I2VGenXLPipeline:
             store_id = (("path", os.path.abspath(store.output_dir)) if store.output_dir is not None else ("store", store))
         else:
             raise ValueError("need `latent_store` or `ddim_inv_latents_path`")
+        if getattr(self.scheduler, "multistep", False):
+            # a multistep edit reads the inversion at its own timesteps (25 steps: 961, 921, ..., 1, every other timestep of
+            # a 50-step inversion); a store that lacks one is refused before anything runs rather than at that step
+            self.scheduler.set_timesteps(num_inference_steps, device=dev)
+            missing = [t for t in self.scheduler.timesteps.tolist()[ddim_init_latents_t_idx:] if t not in store]
+            if missing:
+                raise ValueError(f"the inversion store lacks the source latents of timestep(s) {missing} of the "
+                                 f"{num_inference_steps}-step {type(self.scheduler).__name__} schedule: invert with a number "
+                                 "of steps whose timesteps include them (e.g. 50 for a 25-step edit)")
         if source_features is not None:
             source_features.bind(store_id, ddim_inv_prompt_embeds, ddim_inv_image_embeddings, ddim_inv_image_latents,
                                  target_fps, (latents.shape[2], latents.shape[3], latents.shape[4]), self.unet)
@@ -749,7 +769,7 @@ class I2VGenXLPipeline:
                     v = self.unet(torch.cat([st.latents, st.latents]), st.g_t, cond=st.cond2,
                                   shared_edit_prefix=st.shared_prefix, **replay)[0]
                     st.scheduler.step(v[0:1], None, st.latents, eta=st.eta, model_output_cond=v[1:2], out=st.latents,
-                                      coef_dev=st.g_coef, variance_noise=st.g_noise)
+                                      coef_dev=st.g_coef, variance_noise=st.g_noise, x0_prev=st.x0_prev)
                 return body
             site = self._prune_site(flags) if st.prune_source else None
             lo = 0 if site is not None else 1  # the pruned forward returns [uncond, cond] only
@@ -758,7 +778,7 @@ class I2VGenXLPipeline:
                 v = self.unet(torch.cat([st.g_src, st.latents, st.latents]), st.g_t, cond=st.cond3,
                               shared_edit_prefix=st.shared_prefix, prune_source_after=site)[0]
                 st.scheduler.step(v[lo:lo + 1], None, st.latents, eta=st.eta, model_output_cond=v[lo + 1:lo + 2],
-                                  out=st.latents, coef_dev=st.g_coef, variance_noise=st.g_noise)
+                                  out=st.latents, coef_dev=st.g_coef, variance_noise=st.g_noise, x0_prev=st.x0_prev)
             return body
         if not two_branch:
             st.g_src.copy_(st.store.get(t, device=st.latents.device), non_blocking=True)

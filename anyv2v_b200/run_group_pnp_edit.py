@@ -26,7 +26,7 @@ from .config import OmegaConf
 from .latent_store import LatentStore, load_ddim_latents_at_t
 from .pipeline import I2VGenXLPipeline, frame_position_latents
 from .pnp_utils import register_conv_injection, register_spatial_attention_pnp, register_temp_attention_pnp
-from .schedulers import DDIMScheduler
+from .schedulers import DDIMScheduler, DPMSolverMultistepScheduler
 
 logger = logging.getLogger(__name__)
 
@@ -77,10 +77,32 @@ def synthetic_conditioning(n_frames: int, h: int, w: int, cross_dim: int, seed: 
 
 
 def config_suffix(config) -> str:
-    """reference :154-167."""
-    return ("ddim_init_latents_t_idx_" + str(config.ddim_init_latents_t_idx) + "_nsteps_" + str(config.n_steps) + "_cfg_"
-            + str(config.cfg) + "_pnpf" + str(config.pnp_f_t) + "_pnps" + str(config.pnp_spatial_attn_t) + "_pnpt"
-            + str(config.pnp_temp_attn_t))
+    """reference :154-167; an edit with ``scheduler: dpmsolver++`` adds "_dpmsolver++", so that it does not overwrite the
+    DDIM edit of the same settings."""
+    suffix = ("ddim_init_latents_t_idx_" + str(config.ddim_init_latents_t_idx) + "_nsteps_" + str(config.n_steps) + "_cfg_"
+              + str(config.cfg) + "_pnpf" + str(config.pnp_f_t) + "_pnps" + str(config.pnp_spatial_attn_t) + "_pnpt"
+              + str(config.pnp_temp_attn_t))
+    return suffix + ("" if scheduler_name(config) == "ddim" else "_" + scheduler_name(config))
+
+
+#: the edit schedulers of the optional config key ``scheduler``
+EDIT_SCHEDULERS = ("ddim", "dpmsolver++")
+
+
+def scheduler_name(config) -> str:
+    name = str(config.get("scheduler", "ddim") if hasattr(config, "get") else getattr(config, "scheduler", "ddim"))
+    if name not in EDIT_SCHEDULERS:
+        raise ValueError(f"config key `scheduler`: {name!r} is not one of {list(EDIT_SCHEDULERS)}")
+    return name
+
+
+def edit_scheduler(ddim_scheduler, config):
+    """the scheduler the edit samples with: ``scheduler: ddim`` (the default) the runner's DDIMScheduler, ``dpmsolver++`` a
+    DPMSolverMultistepScheduler on the same config.  The inversion the edit reads stays DDIM: its store must hold every
+    timestep of the edit's schedule (a 50-step inversion serves a 25-step DPM-Solver++ edit)."""
+    if scheduler_name(config) == "ddim":
+        return ddim_scheduler
+    return DPMSolverMultistepScheduler.from_config(ddim_scheduler.config)
 
 
 def load_source_frames(config):
@@ -139,6 +161,7 @@ class SharedSourceFeatures:
 
 
 def edit_one(pipe, ddim_scheduler, config, device, rank_seed_offset: int = 0, source_features=None):
+    ddim_scheduler = edit_scheduler(ddim_scheduler, config)
     config.video_path = os.path.join(config.video_dir, config.video_name + ".mp4")
     config.video_frames_path = os.path.join(config.video_dir, config.video_name)
     config.edited_first_frame_path = os.path.join(config.data_dir, config.edited_first_frame_path)

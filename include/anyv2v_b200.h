@@ -83,6 +83,27 @@ typedef struct {
 } av2v_ddim_eta_args;
 int av2v_ddim_step_eta_f16(const av2v_ddim_eta_args* a, av2v_stream_t stream);
 
+/* CFG combine + one DPM-Solver++(2M) step t -> s (v-prediction; DPMSolverMultistepScheduler, Lu et al. 2022 Alg. 2):
+ *   v   = v_edit ? v_neg + g*(v_edit - v_neg) : v_neg        (rounded as K7 rounds it)
+ *   x0  = fp16(alpha*x - sigma*v)                            -> written to x0_prev (in place, for the next step)
+ *   D   = c != 0 ? x0 + c*(x0 - x0_prev) : x0                (c = 0: first-order step, x0_prev is not read)
+ *   out = fp16(a*x + b*D)
+ * alpha, sigma: of t; a = sigma_s/sigma_t; b = -alpha_s*(exp(-h) - 1), h = lambda_s - lambda_t; c = h/(2*h_prev).
+ * Between the two fp16 roundings every operation is one fp32 rounding in the order written (no FMA contraction). */
+typedef struct {
+  const void* x;      /* current latents, n fp16 */
+  const void* v_neg;  /* model output (uncond chunk when CFG is on), n fp16 */
+  const void* v_edit; /* cond chunk, or NULL for no CFG */
+  void* x0_prev;      /* n fp16: the previous step's x0 in, this step's x0 out; must not alias the other operands */
+  void* out;          /* n fp16; may alias x */
+  int64_t n;
+  float guidance;
+  float alpha, sigma, a, b, c;
+  const float* coef_dev; /* optional device pointer to {alpha, sigma, a, b, c, guidance}, read INSTEAD of the by-value
+                            fields, so that one captured CUDA graph can be replayed for every step */
+} av2v_dpmpp2m_args;
+int av2v_dpmpp2m_step_f16(const av2v_dpmpp2m_args* a, av2v_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------------------
  * K6  GroupNorm (+ optional SiLU), channels-last.
  * Replaces: pnp_utils.py:48-49,92,104 (norm1/norm2 + nonlinearity) and every GroupNorm of the UNet
