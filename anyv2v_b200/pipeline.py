@@ -19,6 +19,7 @@ and ``vae=`` attached — the reference's raw inputs (prompt strings, PIL first 
 """
 from __future__ import annotations
 
+import gc
 import logging
 import os
 from types import SimpleNamespace
@@ -65,9 +66,17 @@ class _GraphedIteration:
             return
         if self.graph is None:
             g = torch.cuda.CUDAGraph()
-            # thread_local: the latent-store writer thread may call cudaEventSynchronize while this thread captures
-            with torch.cuda.graph(g, pool=self.pool, capture_error_mode="thread_local"):
-                self.body()
+            # no cyclic garbage collection inside the capture: a finished loop's state is a reference cycle (its iterations'
+            # bodies close over it), and collecting it there would destroy its CUDA graphs, which invalidates the capture
+            gc_was_on = gc.isenabled()
+            gc.disable()
+            try:
+                # thread_local: the latent-store writer thread may call cudaEventSynchronize while this thread captures
+                with torch.cuda.graph(g, pool=self.pool, capture_error_mode="thread_local"):
+                    self.body()
+            finally:
+                if gc_was_on:
+                    gc.enable()
             self.graph = g
         self.graph.replay()
 

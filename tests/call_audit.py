@@ -5,9 +5,11 @@ actually passes.
 goes through ``ops.<name>(...)``, so the package itself is untouched.  For each call the wrapper
 
 1. snapshots every input that shares storage with what the call writes (``out``; ``freeu``'s ``hidden``, scaled in place;
-   ``ddim_step`` with ``out = x``; a residual that is also the output) — the contract must see the inputs the kernel saw;
+   ``dpmpp2m_step``'s ``x0_prev``, read and then overwritten; ``ddim_step`` with ``out = x``; a residual that is also the
+   output) — the contract must see the inputs the kernel saw;
 2. runs the wrapped op (the sm_90a kernel, or under ``emulated_ops`` its contract) and synchronises;
-3. evaluates the op's contract (tests/kernel_contracts.py ``*_exact``, tests/freeu_ref.py, tests/sampling_ref.py) in
+3. evaluates the op's contract (tests/kernel_contracts.py ``*_exact``, tests/freeu_ref.py, tests/sampling_ref.py,
+   tests/dpm_solver_ref.py, tests/source_cache_ref.py, tests/vae_tiling_ref.py) in
    float64 on the inputs' device, on a seeded subset of the call's independent units, each unit addressed exactly as the
    kernel addressed it (rowbias row m // rows_per_rowbias, the residual row, the output slot, the branch strides):
 
@@ -15,12 +17,15 @@ goes through ``ops.<name>(...)``, so the package itself is untouched.  For each 
        conv3x3, upsample      frames: first, last and 2 seeded frames; every output slot
        tconv3                 clips: first and last
        attention (rows)       query sequences b (keys b // kv_batch_div): first, last and 2 seeded; all heads, rows, branches
-       attention (frames),    pixels of a clip: first, last and 254 seeded per clip; all frames, heads and branches
-       temporal_attention_fused
+       attention (frames),    pixels of a clip: first, last and 254 seeded per clip (edit clip c of a qksrc call: those of
+       temporal_attention_    its source clip c mod clips / 2); all frames, heads and branches
+       fused(_qksrc)
        groupnorm              samples: first, last and 2 seeded
        ddim_step(_eta)        every element, bit for bit
+       dpmpp2m_step           every element of both stores (out and x0_prev), bit for bit
        freeu                  every element: backbone half bit-exact with torch's fp16 ``x * b``, the other half untouched,
                               the filtered skip within the FreeU bound;
+       tile_stitch            images: first, last and 1 seeded; every element, bit for bit, from the call's own tiles
 
 4. compares with the op's element-wise bound (tests/ulp_check.py) and records op, argument signature, worst error in fp16
    ulps and the smallest margin.  Failures are collected, not raised, so that one pass shows every bad call.  The same
@@ -28,8 +33,8 @@ goes through ``ops.<name>(...)``, so the package itself is untouched.  For each 
    over the whole pass: a store that rounds in one direction stays inside every call's bound but not inside that mean.
 
 ``perturb(op, index, args, out)`` runs after the op and before the check, so a test can corrupt one call's output (the
-negative controls of tests/test_call_audit_cpu.py); ``snapshot_after=True`` takes the snapshots after the call instead of
-before, which must make the in-place ops fail.
+negative controls of tests/test_call_audit_cpu.py and tests/test_call_audit_passes_cpu.py); ``snapshot_after=True`` takes
+the snapshots after the call instead of before, which must make the in-place ops fail.
 """
 from __future__ import annotations
 
@@ -39,16 +44,21 @@ from dataclasses import dataclass, field
 
 import torch
 
+import dpm_solver_ref
 import freeu_ref
 import kernel_contracts as kc
 import sampling_ref
+import source_cache_ref
+import vae_tiling_ref
 from bias_check import Moments, moments
 from ulp_check import (KAPPA_ATTN, KAPPA_FREEU, KAPPA_GEGLU, KAPPA_GEMM, KAPPA_NORM, cond_attention, cond_conv_abs, cond_freeu,
                        cond_geglu, cond_groupnorm, cond_layernorm, cond_linear, measure, ulp16)
 
-AUDITED = ("linear", "conv3x3", "upsample2x_conv3x3", "tconv3", "attention", "temporal_attention_fused", "groupnorm",
-           "layernorm", "ddim_step", "ddim_step_eta", "freeu")
+AUDITED = ("linear", "conv3x3", "upsample2x_conv3x3", "tconv3", "attention", "temporal_attention_fused",
+           "temporal_attention_fused_qksrc", "groupnorm", "layernorm", "ddim_step", "ddim_step_eta", "dpmpp2m_step", "freeu",
+           "tile_stitch")
 LAUNCHES = {"upsample2x_conv3x3": 4}  # kernel launches per call; 1 for the others
+_WRITTEN_IN_PLACE = {"freeu": "hidden", "dpmpp2m_step": "x0_prev"}  # written arguments besides ``out``
 
 ROWS_ALL = 8192      # linear / layernorm: every row up to this M
 ROWS_TILE = 128      # ... else the first and last tile of this many rows
@@ -139,7 +149,7 @@ class CallAudit:
             p = sig.bind(*args, **kwargs)
             p.apply_defaults()
             p = dict(p.arguments)
-            written = [t for t in (p.get("out"), p.get("hidden") if name == "freeu" else None) if t is not None]
+            written = [t for t in (p.get("out"), p.get(_WRITTEN_IN_PLACE.get(name))) if t is not None]
             keys = {_storage_key(t) for t in written}
             cache = {}
 
@@ -155,8 +165,8 @@ class CallAudit:
                 self.perturb(name, index, p, out)
             if self.snapshot_after:
                 snap = snapshot()
-            if name == "freeu":
-                snap["_hidden_after"] = p["hidden"]
+            if name in _WRITTEN_IN_PLACE:  # the live tensor, for the check of what the call wrote into it
+                snap["_after"] = p[_WRITTEN_IN_PLACE[name]]
             self.launches += LAUNCHES.get(name, 1)
             n0 = kc._launches  # the contracts count launches when they stand in for the kernels; the audit's own evaluations must not
             try:
@@ -345,8 +355,11 @@ class CallAudit:
             parts.append((f"groupnorm sample {s}", out[s:s + 1], ref, cond, KAPPA_NORM))
             del ref, cond
         chans = f"C={C1}" if x2 is None else f"C={C1}+{C - C1}"
-        sig = f"groupnorm n={n} rows={rows} {chans} groups={p['groups']} eps={p['eps']:g}" + (" silu" if p["silu"] else "")
-        attrs = dict(n=n, rows=rows, C=C, two_source=x2 is not None, silu=bool(p["silu"]), eps=p["eps"], groups=p["groups"])
+        part = p["partition_samples"]
+        sig = (f"groupnorm n={n} rows={rows} {chans} groups={p['groups']} eps={p['eps']:g}" + (" silu" if p["silu"] else "")
+               + (f" partition_samples={part}" if part else ""))
+        attrs = dict(n=n, rows=rows, C=C, two_source=x2 is not None, silu=bool(p["silu"]), eps=p["eps"], groups=p["groups"],
+                     partition_samples=part)
         return self._record(index, "groupnorm", sig, attrs, f"samples {samples.tolist()} of {n}", parts)
 
     def _check_layernorm(self, index, p, out):
@@ -374,8 +387,8 @@ class CallAudit:
         heads, seq, batch, n_v, scale = p["heads"], p["seq"], p["batch"], p["n_v"], p["scale"]
         C = heads * 64
         ldv, ldo = v.stride(0), out.stride(0)
-        vrows = p["v_branch_stride"] // ldv if n_v == 3 else 0
-        orows = p["o_branch_stride"] // ldo if n_v == 3 else 0
+        vrows = p["v_branch_stride"] // ldv if n_v > 1 else 0  # n_v = 3: [source, uncond, cond]; n_v = 2: [uncond, cond]
+        orows = p["o_branch_stride"] // ldo if n_v > 1 else 0
         cond_fn = cond_attention(scale)
         parts = []
         if not p["frames_mode"]:
@@ -435,6 +448,23 @@ class CallAudit:
                             f"{P} of {HW} pixels per clip, {clips} clips",
                             [("temporal attention fused", out[flat, :C], ref, cond, KAPPA_ATTN)])
 
+    def _check_temporal_attention_fused_qksrc(self, index, p, out):
+        x, qk_src, wqkv, heads, F_, HW, clips, scale = p["x"], p["qk_src"], p["wqkv"], p["heads"], p["F"], p["HW"], p["clips"], p["scale"]
+        C = heads * 64
+        idx, P = self._attn_frames_rows(index, clips, F_, HW, clips // 2)  # edit clip c at the pixels of source clip c % (clips/2)
+        flat = _idx(idx.reshape(-1), x)
+        src = _idx(idx[:clips // 2].reshape(-1), qk_src)  # the source clips' rows: source clip c is laid out as edit clip c
+        dummy = torch.empty((flat.numel(), C), dtype=torch.float16, device=x.device)
+        ref, cond = source_cache_ref.temporal_attention_fused_qksrc_exact(
+            x[flat], qk_src[src], wqkv, heads, F_, P, clips, dummy, scale, cond=cond_attention(scale, rounded_operands=True))
+        n = src.numel()
+        got = out[flat, :C]
+        parts = [(f"temporal attention fused qksrc branch {br}", got[br * n:(br + 1) * n], ref[br * n:(br + 1) * n],
+                  cond[br * n:(br + 1) * n], KAPPA_ATTN) for br in range(2)]
+        sig = f"temporal_attention_fused_qksrc clips={clips} F={F_} HW={HW} heads={heads} Cx={x.shape[1]}"
+        return self._record(index, "temporal_attention_fused_qksrc", sig, dict(clips=clips, F=F_, HW=HW, heads=heads),
+                            f"{P} of {HW} pixels per clip, {clips} clips", parts)
+
     def _check_ddim_step(self, index, p, out):
         want = kc.ddim_step(p["x"], p["v_neg"], p["v_edit"], p["guidance"], p["ca"], p["cb"], p["cc"], p["cd"],
                             inverse=p["inverse"], coef_dev=p["coef_dev"])
@@ -450,8 +480,21 @@ class CallAudit:
         return self._record(index, "ddim_step_eta", sig, dict(n=p["x"].numel()), "all",
                             [("ddim_step_eta", out.reshape(-1), want.reshape(-1))])
 
+    def _check_dpmpp2m_step(self, index, p, out):
+        x0_prev = p["x0_prev"].clone()  # the snapshot of the previous x0; the contract overwrites it with this step's
+        want = dpm_solver_ref.dpmpp2m_step(p["x"], p["v_neg"], p["v_edit"], x0_prev, p["guidance"], p["alpha"], p["sigma"],
+                                           p["a"], p["b"], p["c"], coef_dev=p["coef_dev"])
+        c = float(p["c"] if p["coef_dev"] is None else p["coef_dev"][4])
+        order = 1 if c == 0.0 else 2
+        cfg = p["v_edit"] is not None
+        in_place = p["out"] is not None and _storage_key(p["out"]) == _storage_key(p["x"])  # the snapshots share storage too
+        sig = f"dpmpp2m_step n={p['x'].numel()} order={order}" + (" cfg" if cfg else "") + (" in-place" if in_place else "")
+        return self._record(index, "dpmpp2m_step", sig, dict(n=p["x"].numel(), order=order, cfg=cfg, in_place=in_place), "all",
+                            [("dpmpp2m_step out", out.reshape(-1), want.reshape(-1)),
+                             ("dpmpp2m_step x0_prev", p["_after"].reshape(-1), x0_prev.reshape(-1))])
+
     def _check_freeu(self, index, p, out):
-        h0, h1, skip, b, s = p["hidden"], p["_hidden_after"], p["skip"], p["b"], p["s"]
+        h0, h1, skip, b, s = p["hidden"], p["_after"], p["skip"], p["b"], p["s"]
         half = h0.shape[-1] // 2
         s32 = float(torch.tensor(s, dtype=torch.float32))
         ref = freeu_ref.fourier_filter_closed_form(skip.double(), s32)
@@ -461,6 +504,18 @@ class CallAudit:
         NF, H, W, Cs = skip.shape
         sig = f"freeu NF={NF} {H}x{W} Ch={h0.shape[-1]} Cs={Cs} b={b:g} s={s:g}"
         return self._record(index, "freeu", sig, dict(NF=NF, H=H, W=W, Ch=h0.shape[-1], Cs=Cs), "all", parts)
+
+    def _check_tile_stitch(self, index, p, out):
+        tiles = p["tiles"]
+        geo = [p[k] for k in ("H", "W", "tile", "step", "blend", "row_limit")]
+        N, rows, cols, C = len(tiles), len(tiles[0]), len(tiles[0][0]), tiles[0][0][0].shape[0]
+        images = unit_subset(N, 1, self._seed(index))
+        parts = [(f"tile_stitch image {n}", out[n], vae_tiling_ref.stitch_closed_form([tiles[n]], *geo)[0])
+                 for n in images.tolist()]
+        H, W, tile, step, blend, row_limit = geo
+        sig = f"tile_stitch N={N} C={C} {H}x{W} tiles={rows}x{cols} tile={tile} step={step} blend={blend} row_limit={row_limit}"
+        return self._record(index, "tile_stitch", sig, dict(N=N, C=C, H=H, W=W, rows=rows, cols=cols),
+                            f"images {images.tolist()} of {N}", parts)
 
 
 def _product_signatures():

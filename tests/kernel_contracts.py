@@ -268,6 +268,8 @@ def _attention(q, k, v, heads, seq, batch, out, scale, n_v, v_branch_stride, o_b
         o = torch.einsum("...hqk,...khd->...qhd", p, vh.double())
         return o, (None if cond is None else cond(p, qh.double(), kh.double(), vh.double(), o))
 
+    # n_v = 3: V / out of [source, uncond, cond]; n_v = 2: of [uncond, cond] (a step replayed from cached source Q / K).
+    # Either way branch b reads V and writes out at b * its branch stride, with the P of the one Q / K
     branches = range(n_v)
     if not frames_mode:
         div = kv_batch_div if kv_batch_div > 0 else 1
@@ -275,8 +277,8 @@ def _attention(q, k, v, heads, seq, batch, out, scale, n_v, v_branch_stride, o_b
         kvb = batch // div
         qh = q[:batch * seq, :C].reshape(batch, seq, heads, 64)
         kh = k[:kvb * nk, :C].reshape(kvb, nk, heads, 64).repeat_interleave(div, dim=0)
-        vrows = v_branch_stride // ldv if n_v == 3 else 0
-        orows = o_branch_stride // ldo if n_v == 3 else 0
+        vrows = v_branch_stride // ldv if n_v > 1 else 0
+        orows = o_branch_stride // ldo if n_v > 1 else 0
         for b in branches:
             vh = v[b * vrows:b * vrows + kvb * nk, :C].reshape(kvb, nk, heads, 64).repeat_interleave(div, dim=0)
             o, c = sdpa(qh, kh, vh)
@@ -288,8 +290,8 @@ def _attention(q, k, v, heads, seq, batch, out, scale, n_v, v_branch_stride, o_b
         rows = clips * Fr * HW
         to_seq = lambda t: t.reshape(clips, Fr, HW, heads, 64).permute(0, 2, 1, 3, 4)  # [clips, HW, F, heads, 64]
         qh, kh = to_seq(q[:rows, :C]), to_seq(k[:rows, :C])
-        vrows = v_branch_stride // ldv if n_v == 3 else 0
-        orows = o_branch_stride // ldo if n_v == 3 else 0
+        vrows = v_branch_stride // ldv if n_v > 1 else 0
+        orows = o_branch_stride // ldo if n_v > 1 else 0
         for b in branches:
             vh = to_seq(v[b * vrows:b * vrows + rows, :C])
             o, c = sdpa(qh, kh, vh)

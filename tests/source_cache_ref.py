@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE — the contracts of the kernel calls a PnP step replayed from a SourceFeatureCache makes, restated on top of
-tests/kernel_contracts.py: attention with n_v = 2 (the two edit branches of the n_v = 3 call: each branch is n_v = 1 attention
-with the source's Q / K), the fused temporal attention with Q / K from a separate source tensor, and GroupNorm with an explicit
-partition (whose exact statistics do not depend on it).  ``patch_ops`` swaps them in next to the ``emulated_ops`` fixture;
+tests/kernel_contracts.py: attention with n_v = 2 (the two edit branches of the n_v = 3 call, which kernel_contracts states
+directly), the fused temporal attention with Q / K from a separate source tensor, and GroupNorm with an explicit partition
+(whose exact statistics do not depend on it).  ``patch_ops`` swaps them in next to the ``emulated_ops`` fixture;
 tests/test_gpu_source_cache.py checks the kernels against them."""
 from __future__ import annotations
 
@@ -10,44 +10,8 @@ import torch
 import kernel_contracts as kc
 
 
-def _branch(t, b, stride):
-    """rows of branch b of a 2-D token matrix whose branches start `stride` elements apart"""
-    ld = t.stride(0)
-    assert stride % ld == 0, "branch strides are whole rows"
-    return t[b * (stride // ld):]
-
-
-def attention(q, k, v, heads, seq, batch, out, scale=0.125, n_v=1, v_branch_stride=0, o_branch_stride=0, frames_mode=False,
-              HW=0, seq_kv=0, kv_batch_div=0):
-    if n_v != 2:
-        return kc.attention(q, k, v, heads, seq, batch, out, scale, n_v, v_branch_stride, o_branch_stride, frames_mode, HW,
-                            seq_kv, kv_batch_div)
-    for b in range(2):
-        kc.attention(q, k, _branch(v, b, v_branch_stride), heads, seq, batch, _branch(out, b, o_branch_stride), scale,
-                     frames_mode=frames_mode, HW=HW, seq_kv=seq_kv, kv_batch_div=kv_batch_div)
-    return out
-
-
-def attention_exact(q, k, v, heads, seq, batch, out, scale=0.125, n_v=1, v_branch_stride=0, o_branch_stride=0,
-                    frames_mode=False, HW=0, seq_kv=0, kv_batch_div=0, cond=None):
-    """kernel_contracts.attention_exact, also at n_v = 2"""
-    if n_v != 2:
-        return kc.attention_exact(q, k, v, heads, seq, batch, out, scale, n_v, v_branch_stride, o_branch_stride, frames_mode,
-                                  HW, seq_kv, kv_batch_div, cond)
-    C = heads * 64
-    ref = torch.full((out.shape[0], C), float("nan"), dtype=torch.float64, device=q.device)
-    cnd = torch.full_like(ref, float("nan")) if cond is not None else None
-    orows = o_branch_stride // out.stride(0)
-    for b in range(2):
-        ob = _branch(out, b, o_branch_stride)
-        r, c = kc.attention_exact(q, k, _branch(v, b, v_branch_stride), heads, seq, batch, ob, scale, frames_mode=frames_mode,
-                                  HW=HW, seq_kv=seq_kv, kv_batch_div=kv_batch_div, cond=cond)
-        n = ob.shape[0]
-        keep = ~torch.isnan(r[:, 0])
-        ref[b * orows:b * orows + n][keep] = r[keep]
-        if cond is not None:
-            cnd[b * orows:b * orows + n][keep] = c[keep]
-    return ref, cnd
+attention = kc.attention
+attention_exact = kc.attention_exact
 
 
 def _tattn_qksrc_operands(x, qk_src, wqkv, heads, F_, HW, clips, out, scale):

@@ -63,6 +63,45 @@ def test_group_runners_end_to_end(tmp_path):
     assert os.path.exists(saved) and torch.equal(torch.load(saved), res[0].cpu())
 
 
+def test_capture_outlives_a_loop_state_that_dies_during_it():
+    """A finished loop's state is a reference cycle (its iterations' bodies close over it) holding CUDA graphs.  When it
+    becomes garbage while another iteration captures, the cyclic collector must not free it there: destroying a graph
+    inside a capture invalidates the capture.  It is freed at the next collection outside the capture."""
+    import gc
+    import weakref
+    from anyv2v_b200.pipeline import _GraphedIteration
+
+    def loop_state():
+        st = SimpleNamespace(x=torch.zeros(8, device=dev))
+        st.it = _GraphedIteration(lambda: st.x.add_(1))  # st -> it -> body -> st
+        for _ in range(2):
+            st.it.run()                                # eager, then captured: the cycle holds a CUDAGraph
+        return st
+    holder = [loop_state()]
+    gone = weakref.ref(holder[0].it)
+    x, seen = torch.zeros(1024, device=dev), []
+
+    def body():
+        seen.append(gc.isenabled())
+        if torch.cuda.is_current_stream_capturing():
+            holder.clear()                             # the old state becomes garbage inside the capture
+            _ = [[] for _ in range(2000)]              # ... and a collection falls due
+        x.add_(1)
+    it = _GraphedIteration(body)
+    threshold = gc.get_threshold()
+    gc.set_threshold(1)
+    try:
+        for _ in range(3):
+            it.run()                                   # eager, capture + replay, replay
+    finally:
+        gc.set_threshold(*threshold)
+    torch.cuda.synchronize()
+    assert seen == [True, False] and gc.isenabled()
+    assert torch.all(x == 3)
+    gc.collect()
+    assert gone() is None
+
+
 def test_cuda_graph_replay_equals_eager():
     """A captured loop iteration replayed with new device-resident scalars == the same kernels launched eagerly."""
     from anyv2v_b200.pipeline import I2VGenXLPipeline

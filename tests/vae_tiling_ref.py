@@ -5,7 +5,8 @@
    ``DiffusersTiling(vae)`` wraps an oracle/vae_ref.py AutoencoderKL with diffusers' attributes, `encode` / `decode` dispatch,
    `tiled_encode`, `tiled_decode`, and the in-place `blend_v` / `blend_h` loop (``blend_loop``).
 2. Contract of `ops.tile_stitch` (csrc/vae_tiles.cu): ``stitch_closed_form``, each output element from at most four raw tiles,
-   evaluated with the same torch fp16 rounding sequence as the loop.
+   evaluated with the same torch fp16 rounding sequence as the loop, on the tiles' device; ``tile_stitch`` stands in for the
+   kernel under ``patch_ops``.
 3. Geometry: ``geometry``, the tile starts / extents, blend extent and row limit of the loop, stated from diffusers' formulas.
 """
 from __future__ import annotations
@@ -14,6 +15,7 @@ from types import SimpleNamespace
 
 import torch
 
+import kernel_contracts
 from oracle.vae_ref import DiagonalGaussianDistribution
 
 
@@ -149,7 +151,7 @@ def _blend(a, b, pos, e, dim):
     shape = [1] * a.dim()
     shape[dim] = len(pos)
     r = torch.tensor([p / e for p in pos], dtype=torch.float64)
-    wa, wb = (1 - r).float().view(shape), r.float().view(shape)
+    wa, wb = (1 - r).float().view(shape).to(a.device), r.float().view(shape).to(a.device)
     return ((a.float() * wa).half().float() + (b.float() * wb).half().float()).half()
 
 
@@ -188,7 +190,17 @@ def stitch_closed_form(tiles, H, W, tile, step, blend, row_limit):
     return torch.stack(out)
 
 
+def tile_stitch(tiles, H, W, tile, step, blend, row_limit, out=None):
+    """ops.tile_stitch as one counted launch of the closed form (into ``out`` when it is given)"""
+    y = stitch_closed_form(tiles, H, W, tile, step, blend, row_limit)
+    kernel_contracts._count()
+    if out is None:
+        return y
+    out.copy_(y)
+    return out
+
+
 def patch_ops(monkeypatch):
     """ops.tile_stitch -> the contract for one test (use together with the emulated_ops fixture, which patches the other ops)"""
     from anyv2v_b200 import ops
-    monkeypatch.setattr(ops, "tile_stitch", stitch_closed_form)
+    monkeypatch.setattr(ops, "tile_stitch", tile_stitch)
